@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Benchmark of the STAR denoising hot path on B200 (driver contract: one JSON line on rank 0).
+"""Benchmark of the STAR denoising hot path on H100 (one JSON result line on rank 0).
 
 Metric (BASELINE.json): upscaled frames/sec, 4x 240p->960p I2VGen-XL, 32-frame chunks, 50 steps.
   * workload (N=1): BASELINE.json configs[1] -- one 32-frame chunk at latent 122x216 (240p -> 960p
@@ -15,7 +15,7 @@ Metric (BASELINE.json): upscaled frames/sec, 4x 240p->960p I2VGen-XL, 32-frame c
     chunk, so the clip has 16(N+1) unique frames: that rate is config.unique_frames_per_s.
   * e2e: the same metric through VideoToVideo_sr.denoise_latents() from pinned HOST tensors, one
     1-step call per "step": H2D of latent + text embeddings and D2H of the result inside the timing.
-  * gpu_reference (N=1): the UNMODIFIED reference modules (.half() + autocast, xformers -> SDPA) timed on the same B200 on
+  * gpu_reference (N=1): the UNMODIFIED reference modules (.half() + autocast, xformers -> SDPA) timed on the same GPU on
     the same shape in a child process (tools/ref_gpu.py; needs the staged tree oracle/_ref, see oracle/stage_reference.py):
     the denominator of the north-star's ">= 8x the reference's single-GPU PyTorch frames/sec".
   * config3 (N>=6): BASELINE config 3 -- a 72-frame clip = chunks 32/32/40 -- on the same ranks with the CFG-branch split
@@ -57,13 +57,15 @@ def parse():
     ap.add_argument("--small", action="store_true", help="reduced model (debug only; not a valid bench line)")
     ap.add_argument("--workload", default="denoise", choices=["denoise", "vae", "cogvideox"],
                     help="denoise = BASELINE config 2 (the driver's line); vae = config 5 decode sweep; cogvideox = config 4 DiT step")
-    ap.add_argument("--lib", default="", help="A/B: load this variant of libstar_sm100.so (tools/build_variant.py); not a valid bench line")
+    ap.add_argument("--lib", default="", help="A/B: load this variant of libstar_sm100.so; not a valid bench line")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write the denoised latent of the timed steps to DIR/denoised_latent.npy (float32)")
     return ap.parse_args()
 
 
 # ---------------------------------------------------------------------------------- helpers
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -113,23 +115,7 @@ def measured_peaks():
         d = json.load(open(p))
         return {"tflops": d.get("bf16_tflops_sustained", d.get("bf16_tflops")), "hbm_gbs": d.get("hbm_gbs"),
                 "source": "MEASURED_PEAKS.json (bf16_tflops_sustained: kernel timed inside a long step)"}
-    return {"tflops": 1590.0, "hbm_gbs": 6650.0, "source": "fallback (B200_PROFILING.md)"}
-
-
-def ncu_traffic_bytes():
-    """DRAM bytes per launch of the dominant kernel from the committed ncu --set full capture (profiles/)."""
-    path = os.path.join(ROOT, "profiles", "r02_ncu_attn4.txt")
-    if not os.path.isfile(path):
-        path = os.path.join(ROOT, "profiles", "r01_ncu_attn4_split.txt")
-    if not os.path.isfile(path):
-        return None
-    mult = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
-    tot = 0.0
-    for line in open(path):
-        parts = line.split()
-        if len(parts) >= 3 and parts[0] in ("dram__bytes_read.sum", "dram__bytes_write.sum") and parts[1] in mult:
-            tot += float(parts[2]) * mult[parts[1]]
-    return tot or None
+    return {"tflops": 989.0, "hbm_gbs": 3350.0, "source": "H100 SXM data sheet (dense fp16, 700 W); not measured"}
 
 
 def build_model(small, device, seed=2, on_cpu_first=False):
@@ -321,7 +307,7 @@ def time_vae(pipe, latent, F, H, W, dev, ms_per_step, world=1, rank=0, barrier=N
             dec_ms, enc_ms = tt.tolist()
         ok = bool(torch.isfinite(vid).all()) and vid.shape[0] == F
         denoise_s = SCHEDULE_STEPS * ms_per_step / 1e3
-        return {"vae": "star_b200 AutoencoderKLTemporalDecoder (sm_100a kernels), synthetic weights, parity unpinned",
+        return {"vae": "star_b200 AutoencoderKLTemporalDecoder (sm_90a kernels), synthetic weights, parity unpinned",
                 "sharding": "single GPU" if world == 1 else
                             f"3-frame decode windows round-robin over {world} ranks + ONE all-gather of decoded frames; "
                             f"per-frame encode of each rank's share + all-gather of latents",
@@ -335,19 +321,15 @@ def time_vae(pipe, latent, F, H, W, dev, ms_per_step, world=1, rank=0, barrier=N
 
 
 def gpu_reference_block(H, W):
-    """the unmodified reference modules on this B200 (child process, after the product's memory is released)"""
-    staged = os.path.join(ROOT, "oracle", "_ref", "video_to_video", "modules", "unet_v2v.py")
-    recorded = os.path.join(ROOT, "profiles", "r02_ref_gpu_c2.json")
+    """the unmodified reference modules on this GPU (child process, after the product's memory is released)"""
+    import tempfile
+    from oracle.ref_loader import reference_available
     note = {"what": "reference ControlledV2VUNet().half() under torch.autocast('cuda', fp16), xformers.memory_efficient_attention -> "
-                    "F.scaled_dot_product_attention (xformers 0.0.21 has no sm_100 build); same weights / shape as `value`",
-            "recorded_run": "profiles/r02_ref_gpu_c2.json (2 244 ms per forward, 0.1426 frames/s; star 751 ms; parity at this shape)"
-            if os.path.isfile(recorded) else None}
-    if not (os.path.isfile(staged) or os.path.isfile("/root/reference/video_to_video/modules/unet_v2v.py")):
-        return dict(note, unavailable="reference tree not on this box (oracle/_ref is git-ignored; run `python -m oracle.stage_reference` "
-                                      "in the build container before shipping)")
-    out = os.path.join(ROOT, "gpurun_out", "bench_gpu_reference.json")
+                    "F.scaled_dot_product_attention (xformers is not installed); same weights / shape as `value`"}
+    if not reference_available():
+        return dict(note, unavailable="reference tree not present (oracle/_ref is staged by build() where the reference exists)")
+    out = os.path.join(tempfile.mkdtemp(prefix="star_bench_"), "bench_gpu_reference.json")
     try:
-        os.makedirs(os.path.dirname(out), exist_ok=True)
         r = subprocess.run([sys.executable, os.path.join(ROOT, "tools", "ref_gpu.py"), "--no-star", "--no-fp32", "--iters", "3",
                             "--shape", f"{CHUNK},{H},{W}", "--out", out], capture_output=True, text=True, timeout=420)
         d = json.load(open(out))
@@ -366,8 +348,8 @@ VAE_SWEEP = {"540p/720p (720x1280)": (90, 160, 11.0, 17.2), "960p (976x1728)": (
 
 def run_vae_sweep(args):
     """Temporal-VAE decode of 3-frame windows (ref video_to_video_model.py:141-151) at the three BASELINE config-5 output
-    sizes, UNTILED: the largest window peaks at a few GB of the 180 GB HBM, so the reference's (non-existent) spatial tiling
-    is not needed on B200 and the per-window GroupNorm statistics stay exact by construction."""
+    sizes, UNTILED: the largest window peaks at a few GB of the 80 GB HBM, so the reference's (non-existent) spatial tiling
+    is not needed on H100 and the per-window GroupNorm statistics stay exact by construction."""
     from star_b200 import ops
     from star_b200.utils.synth import synth_tensor
     from star_b200.video_to_video.modules.temporal_vae import AutoencoderKLTemporalDecoder
@@ -413,7 +395,7 @@ def run_vae_sweep(args):
             "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f16", "data": "synthetic",
             "config": {"workload": "VAE decode sweep 540p/720p/960p/1080p outputs (value = 976x1728), untiled 3-frame windows",
                        "model": "AutoencoderKLTemporalDecoder (SVD temporal VAE), synthetic weights, PARITY UNPINNED (diffusers absent)",
-                       "l2": "activations (0.43 GB per 128-channel full-resolution tensor) exceed the 126 MB L2"},
+                       "l2": "activations (0.43 GB per 128-channel full-resolution tensor) exceed the 50 MB L2"},
             "clocks": clocks.stop(), "gpu_launches": int(launches), "sweep": rows,
             "roofline": {"kernel": "whole decode (conv / GroupNorm / conv_t3 kernels)", "bound": "hbm",
                          "achieved": mid["algorithmic_gb_per_s"], "peak": peaks["hbm_gbs"], "unit": "GB/s",
@@ -483,6 +465,7 @@ def main():
     barrier()
 
     # ---- timed: exactly K solver steps, device-resident inputs ----------------------------------
+    torch.manual_seed(0)                # the diffusion noise: identical inputs from run to run (--dump-outputs)
     clocks = ClockSampler(local)
     if rank == 0:
         clocks.start()
@@ -499,6 +482,10 @@ def main():
     out_checksum = {"sum": float(out.double().sum()), "abs_mean": float(out.abs().mean()), "finite": out_finite}
     if not out_finite:
         raise SystemExit("bench.py: non-finite values in the denoised latent -- not a valid bench run")
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "denoised_latent.npy"), out.float().cpu().numpy())
     # one more (un-timed) solver step with per-op CUDA events for the roofline / op shares: the event bookkeeping
     # costs host time per launch and must not sit inside the timed region
     ops.trace_begin()
@@ -592,12 +579,10 @@ def main():
         flops = 4.0 * hw0 * hw0 * 64 * batch * heads
         avg = sum(t for _, t in attn_ms) / len(attn_ms)
         ach = flops / (avg * 1e-3) / 1e12
-        roof = {"kernel": "attn4_fwd_kernel (spatial self-attention, finest level, row-split softmax)", "bound": "tensor",
+        roof = {"kernel": "attn_fwd_kernel (spatial self-attention, finest level)", "bound": "tensor",
                 "achieved": ach, "peak": peaks["tflops"], "unit": "TFLOP/s", "frac": ach / peaks["tflops"],
                 "peak_source": peaks["source"], "algorithmic_flops_per_launch": flops, "avg_launch_ms": avg,
-                "launches_timed": len(attn_ms), "traffic": ncu_traffic_bytes(),
-                "traffic_source": "dram__bytes_read+write of one `ncu --set full` capture of this kernel at this shape "
-                                  "(profiles/r02_ncu_attn4.txt); a constant of the kernel, not re-measured per run",
+                "launches_timed": len(attn_ms),
                 "algorithmic_bytes_per_launch": 4.0 * batch * heads * hw0 * 64 * 2,
                 "share_of_step": sum(t for _, t in attn_ms) / sum(per_op.values())}
     if args.trace_out and rank == 0:
@@ -650,7 +635,7 @@ def main():
                                "overlap by 16 frames as in the reference, see unique_frames_per_s",
                        "chunk_frames": chunk_frames, "unique_frames_per_s": unique_value,
                        "parallelism": f"chunk-parallel x{world}, per-step x0 all-gather" if world > 1 else "single GPU",
-                       "l2": "activations (0.54 GB per tensor) exceed the 126 MB L2; no explicit flush",
+                       "l2": "activations (0.54 GB per tensor) exceed the 50 MB L2; no explicit flush",
                        "step": "one solver step = 2 UNet+ControlNet forwards (CFG) + guidance + solver update; the two forwards' common, "
                                "text-independent prefix (stem, first temporal transformer, first ResBlock, first spatial self-attention "
                                "of each network) is evaluated once -- bit-identical outputs (forward_cfg_pair), ~7 % of the step's FLOPs",

@@ -1,4 +1,4 @@
-/* star_sm100.h -- C ABI of libstar_sm100.so (star_b200/csrc), the sm_100a kernel library
+/* star_sm100.h -- C ABI of libstar_sm100.so (star_b200/csrc), the sm_90a (H100) kernel library
  * behind star_b200's drop-in for the STAR denoising hot path.
  *
  * The reference (NJU-PCALab/STAR) has no FFI: every kernel it runs is dispatched by
@@ -29,7 +29,7 @@ int star_version(void);
 const char* star_last_error(void);
 /* number of kernels this library has launched since it was loaded (all streams) */
 long long star_launch_count(void);
-/* Resolve cuTensorMapEncodeTiled, opt kernels into >48 KB shared memory.  Fails on non-sm_100 devices. */
+/* Resolve cuTensorMapEncodeTiled, opt kernels into >48 KB shared memory.  Fails on non-sm_90 devices. */
 int star_init(int device);
 
 /* nn.Linear / Conv2d 1x1 / Conv1d k=1: out[r, n] = sum_k A[r,k] W[n,k] (+bias[n]) (+rowvec[r/rowvec_div, n])

@@ -2,7 +2,7 @@
 
 /root/reference exists only in the build container.  The GPU-side baseline the north-star's ">= 8x the
 reference's single-GPU PyTorch frames/sec" is written against (SURVEY 8d "Reference timed beside it",
-VERDICT r1 item 1) needs the UNMODIFIED reference modules on the B200, so this recipe copies the few files
+VERDICT r1 item 1) needs the UNMODIFIED reference modules on the GPU, so this recipe copies the few files
 oracle/ref_loader.py executes into oracle/_ref/ -- git-ignored (no reference source enters the history), not
 gpurun-ignored (it travels with the snapshot like a built .so).  Nothing is edited; ref_loader's import shims
 are applied at load time exactly as in the container.

@@ -1,4 +1,4 @@
-"""star_b200 -- Blackwell-native (sm_100a) implementation of the STAR
+"""star_b200 -- Hopper-native (sm_90a, H100) implementation of the STAR
 video-super-resolution denoising hot path (NJU-PCALab/STAR,
 video_to_video/: VideoToVideo_sr.test -> GaussianDiffusion.sample_sr ->
 ControlledV2VUNet.forward).  See DESIGN.md."""

@@ -1,4 +1,4 @@
-"""STAR's CogVideoX-5B path (cogvideox-based/) on the sm_100a kernels: the DiT (one layer: DiTLayer; the whole
+"""STAR's CogVideoX-5B path (cogvideox-based/) on the sm_90a kernels: the DiT (one layer: DiTLayer; the whole
 DiffusionTransformer: patch embed, 42 layers with LoRA merged, final layer), the sampling loop (VPSDEDPMPP2MSampler + DynamicCFG +
 DiscreteDenoiser / VideoScaling), the 3-D causal VAE (encoder and decoder), and the frames-to-frames glue of sample_sr.py."""
 from .dit_block import DiTLayer  # noqa: F401

@@ -3,7 +3,7 @@
 Reference (cogvideox-based/): AdaLNMixin.layer_forward (sat/dit_video_concat.py:482-563), the qk-LayerNorm and 3-D
 rotary attention_fn mixins (:570-598, :306-346), SpatialAttention / TemporalLocalAttention (transformer.py:316-348) and
 sat's default SelfAttention / MLP (transformer.py:35-119, :202-312).  Same kernels as the I2VGen-XL path:
-  * fused QKV / dense / MLP GEMMs on the persistent tcgen05 tap-GEMM, with the adaLN gate and residual
+  * fused QKV / dense / MLP GEMMs on the persistent wgmma tap-GEMM, with the adaLN gate and residual
     (``hidden + gate * f(x)``) and the tanh-GELU folded into the epilogue (star_linear_ex),
   * the 3-D full attention over text + T*H*W tokens (48 heads x 64, N = 17 776) on the TMEM-resident flash
     attention kernel (attn4), fed by a fused per-head qk-LayerNorm + rotary kernel,

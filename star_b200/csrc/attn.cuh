@@ -4,284 +4,197 @@
 // replaces xformers.ops.memory_efficient_attention at unet_v2v.py:179/:184 for the
 // spatial self-attention (N = H*W up to 26 352) and the text cross-attention (Nk = 77).
 //
-// One CTA = 128 query rows of one (batch, head).  Warp roles (192 threads):
-//   warp 0     TMA producer: Q once, then K/V tiles (128 keys) through a 3-stage ring
-//   warp 1     TMEM owner + single-thread tcgen05.mma issuer:
-//                S_j  = Q K_j^T   -> TMEM S[j&1]   (128x128 fp32, double buffered)
-//                Op_j = P_j V_j   -> TMEM O[j&1]   (128x64 fp32)
-//   warps 2-5  softmax: thread r owns query row r (TMEM lane r): row max / exp2 / sum with
-//              no cross-thread traffic, P_j written as fp16 into the SWIZZLE_128B K-major smem
-//              layout the PV MMA reads; running output kept in registers and rescaled by
-//              exp2(m_old - m_new) when the partial product is folded in.
-// S_{j+1} is issued before P_j is consumed, so the QK^T of the next tile overlaps the softmax
-// of the current one.
+// One CTA = 128 query rows of one (batch, head).  Warp roles (384 threads):
+//   warpgroup 0      one TMA producer thread: Q once, then K/V tiles (128 keys) through a ring of stages
+//   warpgroups 1, 2  64 query rows each:
+//                      S_j = Q K_j^T            wgmma m64n128k16, both operands K-major in shared memory
+//                      online softmax on the S fragment in registers (two rows per thread, quad shuffles)
+//                      O  += P_j V_j            wgmma m64n64k16 with P as the register A operand (the S
+//                                               accumulator fragment packed to fp16 pairs) and V MN-major
+// Keys beyond Nk are zero-filled by TMA and masked; with `causal` the key tiles past the last query row are skipped.
 #pragma once
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace star {
 
 constexpr int AT_BQ = 128;
 constexpr int AT_BKV = 128;
 constexpr int AT_D = 64;
-constexpr int AT_KV_STAGES = 3;
-constexpr int AT_THREADS = 192;
+constexpr int AT_KV_STAGES = 4;
+constexpr int AT_THREADS = 384;
+constexpr int AT_CONSUMER_WARPS = 8;
 
 struct AttnParams {
     int Nq, Nk;
-    int causal;             // 1: query row q attends keys 0..q only (text tower); honoured by attn_fwd_kernel, not by attn4
+    int causal;             // 1: query row q attends keys 0..q only (text tower)
     int kv_batch_div;       // kv batch index = q batch index / kv_batch_div (text context shared by the frames of a clip)
     float scale_log2;       // softmax scale * log2(e)
     __half* out;
     long long ldo;          // elements between consecutive rows of O
 };
 
-// SINGLE = the whole key range is one KV tile (text cross-attention, Nk = 77): no rings, one S / P / O buffer,
-// 256 TMEM columns and 81 KB of shared memory, so that TWO CTAs are resident per SM -- such a CTA is a strictly
-// serial load -> MMA -> softmax -> MMA -> store chain and only co-resident CTAs overlap it (the general
-// configuration holds one CTA per SM: 1.34 ms for the 26 352-token level, 12 % of the HBM rate).
-template <bool SINGLE>
-struct AttnSmemT {
-    static constexpr int STAGES = SINGLE ? 1 : AT_KV_STAGES;
-    static constexpr int NBUF = SINGLE ? 1 : 2;
-    static constexpr int Q_BYTES = AT_BQ * AT_D * 2;        // 16 KB
-    static constexpr int KV_BYTES = AT_BKV * AT_D * 2;      // 16 KB each
-    static constexpr int P_BYTES = AT_BQ * AT_BKV * 2;      // 32 KB
+struct AttnSmem {
+    static constexpr int TILE = AT_BQ * AT_D * 2;             // 16 KB (Q, and one K or V tile of 128 keys)
     static constexpr int OFF_Q = 0;
-    static constexpr int OFF_K = OFF_Q + Q_BYTES;
-    static constexpr int OFF_V = OFF_K + STAGES * KV_BYTES;
-    static constexpr int OFF_P = OFF_V + STAGES * KV_BYTES;
-    static constexpr int OFF_BAR = OFF_P + NBUF * P_BYTES;
+    static constexpr int OFF_K = OFF_Q + TILE;
+    static constexpr int OFF_V = OFF_K + AT_KV_STAGES * TILE;
+    static constexpr int OFF_BAR = OFF_V + AT_KV_STAGES * TILE;
     static constexpr int TOTAL = OFF_BAR + 256 + 1024;
 };
-using AttnSmem = AttnSmemT<false>;
 
-template <bool SINGLE>
-__global__ void __launch_bounds__(AT_THREADS, SINGLE ? 2 : 1)
+__global__ void __launch_bounds__(AT_THREADS, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                 const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ AttnParams p) {
-    using AttnSmem = AttnSmemT<SINGLE>;
-    constexpr int AT_KV_STAGES = AttnSmem::STAGES;           // shadows the namespace constant
-    constexpr uint32_t TMEM_COLS = SINGLE ? 256 : 512;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + AttnSmem::OFF_BAR);
-    uint64_t* q_full = bars;                 // 1
-    uint64_t* kv_full = bars + 1;            // 3
-    uint64_t* kv_empty = bars + 4;           // 3
-    uint64_t* s_full = bars + 7;             // 2
-    uint64_t* s_empty = bars + 9;            // 2
-    uint64_t* p_full = bars + 11;            // 2
-    uint64_t* p_empty = bars + 13;           // 2
-    uint64_t* o_full = bars + 15;            // 2
-    uint64_t* o_empty = bars + 17;           // 2
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 19);
+    uint64_t* q_full = bars;                           // 1
+    uint64_t* kv_full = bars + 1;                      // AT_KV_STAGES
+    uint64_t* kv_empty = kv_full + AT_KV_STAGES;       // AT_KV_STAGES
 
+    const int wg = threadIdx.x >> 7;
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
     const int q0 = blockIdx.x * AT_BQ;
     const int head = blockIdx.y;
     const int batch = blockIdx.z;
     const int kv_batch = batch / p.kv_batch_div;
-    const int nt = (p.Nk + AT_BKV - 1) / AT_BKV;
+    int nt = (p.Nk + AT_BKV - 1) / AT_BKV;
+    if (p.causal) nt = min(nt, (min(p.Nq, q0 + AT_BQ) + AT_BKV - 1) / AT_BKV);   // keys past the tile's last query
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         tma_prefetch_desc(&tmap_q);
         tma_prefetch_desc(&tmap_k);
         tma_prefetch_desc(&tmap_v);
-    }
-    if (warp == 1) {
-        if (lane == 0) {
-            mbar_init(q_full, 1);
-            for (int s = 0; s < AT_KV_STAGES; ++s) {
-                mbar_init(&kv_full[s], 1);
-                mbar_init(&kv_empty[s], 1);
-            }
-            for (int b = 0; b < 2; ++b) {
-                mbar_init(&s_full[b], 1);
-                mbar_init(&s_empty[b], 128);
-                mbar_init(&p_full[b], 128);
-                mbar_init(&p_empty[b], 1);
-                mbar_init(&o_full[b], 1);
-                mbar_init(&o_empty[b], 128);
-            }
-            fence_barrier_init();
+        mbar_init(q_full, 1);
+        for (int s = 0; s < AT_KV_STAGES; ++s) {
+            mbar_init(&kv_full[s], 1);
+            mbar_init(&kv_empty[s], AT_CONSUMER_WARPS);
         }
-        __syncwarp();
-        tmem_alloc<TMEM_COLS>(tmem_slot);
+        fence_barrier_init();
     }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    const uint32_t tmem_s0 = tmem_base;            // S[b] at columns b*128
-    const uint32_t tmem_o0 = tmem_base + (SINGLE ? 128 : 256);      // O[b] at columns 256 + b*64 (SINGLE: one O at 128)
 
-    if (warp == 0) {
-        if (lane == 0) {
-            mbar_expect_tx(q_full, AttnSmem::Q_BYTES);
+    if (wg == 0) {
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 24;");
+        if (threadIdx.x == 0) {
+            mbar_expect_tx(q_full, AttnSmem::TILE);
             tma_load_3d(smem + AttnSmem::OFF_Q, &tmap_q, q_full, head * AT_D, q0, batch);
+            int s = 0;
+            uint32_t ph = 0;
             for (int j = 0; j < nt; ++j) {
-                const int s = j % AT_KV_STAGES;
-                const uint32_t ph = (j / AT_KV_STAGES) & 1;
                 mbar_wait(&kv_empty[s], ph ^ 1);
-                mbar_expect_tx(&kv_full[s], 2 * AttnSmem::KV_BYTES);
-                tma_load_3d(smem + AttnSmem::OFF_K + s * AttnSmem::KV_BYTES, &tmap_k, &kv_full[s], head * AT_D,
-                            j * AT_BKV, kv_batch);
-                tma_load_3d(smem + AttnSmem::OFF_V + s * AttnSmem::KV_BYTES, &tmap_v, &kv_full[s], head * AT_D,
-                            j * AT_BKV, kv_batch);
+                mbar_expect_tx(&kv_full[s], 2 * AttnSmem::TILE);
+                tma_load_3d(smem + AttnSmem::OFF_K + s * AttnSmem::TILE, &tmap_k, &kv_full[s], head * AT_D, j * AT_BKV, kv_batch);
+                tma_load_3d(smem + AttnSmem::OFF_V + s * AttnSmem::TILE, &tmap_v, &kv_full[s], head * AT_D, j * AT_BKV, kv_batch);
+                if (++s == AT_KV_STAGES) { s = 0; ph ^= 1; }
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            constexpr uint32_t idesc_s = umma_idesc_f16(AT_BQ, AT_BKV, 0, 0);   // S = Q K^T : both K-major
-            constexpr uint32_t idesc_o = umma_idesc_f16(AT_BQ, AT_D, 0, 1);     // O = P V   : V is MN-major
-            const uint32_t q_addr = smem_u32(smem + AttnSmem::OFF_Q);
-            auto issue_s = [&](int j) {
-                const int s = j % AT_KV_STAGES;
-                const int b = j & 1;
-                mbar_wait(&kv_full[s], (j / AT_KV_STAGES) & 1);
-                mbar_wait(&s_empty[b], ((j >> 1) & 1) ^ 1);
-                tc_fence_after();
-                const uint32_t k_addr = smem_u32(smem + AttnSmem::OFF_K + s * AttnSmem::KV_BYTES);
-#pragma unroll
-                for (int k = 0; k < AT_D / 16; ++k) {
-                    umma_f16_ss(tmem_s0 + b * 128, umma_desc_sw128(q_addr + k * 32, 16, 1024),
-                                umma_desc_sw128(k_addr + k * 32, 16, 1024), idesc_s, k > 0 ? 1u : 0u);
-                }
-                umma_commit(&s_full[b]);
-            };
-            mbar_wait(q_full, 0);
-            issue_s(0);
-            for (int j = 0; j < nt; ++j) {
-                if (j + 1 < nt) issue_s(j + 1);
-                const int s = j % AT_KV_STAGES;
-                const int b = j & 1;
-                mbar_wait(&p_full[b], (j >> 1) & 1);
-                mbar_wait(&o_empty[b], ((j >> 1) & 1) ^ 1);
-                tc_fence_after();
-                const uint32_t p_addr = smem_u32(smem + AttnSmem::OFF_P + b * AttnSmem::P_BYTES);
-                const uint32_t v_addr = smem_u32(smem + AttnSmem::OFF_V + s * AttnSmem::KV_BYTES);
-#pragma unroll
-                for (int k = 0; k < AT_BKV / 16; ++k) {
-                    const uint64_t da = umma_desc_sw128(p_addr + (k >> 2) * 16384 + (k & 3) * 32, 16, 1024);
-                    const uint64_t db = umma_desc_sw128(v_addr + k * 2048, 8192, 1024);
-                    umma_f16_ss(tmem_o0 + b * 64, da, db, idesc_o, k > 0 ? 1u : 0u);
-                }
-                umma_commit(&o_full[b]);
-                umma_commit(&kv_empty[s]);
-                umma_commit(&p_empty[b]);
-            }
-        }
-    } else {
-        const int quad = warp & 3;
-        const int r = quad * 32 + lane;
-        const uint32_t lane_off = (uint32_t)(quad * 32) << 16;
-        float m_run = -INFINITY, l_run = 0.f, alpha_prev = 0.f;
-        float o[AT_D];
-#pragma unroll
-        for (int i = 0; i < AT_D; ++i) o[i] = 0.f;
-
-        auto fold_o = [&](int j) {      // o = o * alpha_j + Opart_j
-            const int b = j & 1;
-            mbar_wait(&o_full[b], (j >> 1) & 1);
-            tc_fence_after();
-            uint32_t v[32];
-#pragma unroll
-            for (int c = 0; c < 2; ++c) {
-                tmem_ld32(tmem_o0 + b * 64 + lane_off + c * 32, v);
-                tmem_ld_wait();
-#pragma unroll
-                for (int i = 0; i < 32; ++i) o[c * 32 + i] = o[c * 32 + i] * alpha_prev + __uint_as_float(v[i]);
-            }
-            tc_fence_before();
-            mbar_arrive(&o_empty[b]);
-        };
-
-        for (int j = 0; j < nt; ++j) {
-            const int b = j & 1;
-            const int kbase = j * AT_BKV;
-            const int klim = p.causal ? min(p.Nk, q0 + r + 1) : p.Nk;      // keys [0, klim) are visible to this row
-            const bool tail = (kbase + AT_BKV > klim);
-            mbar_wait(&s_full[b], (j >> 1) & 1);
-            tc_fence_after();
-            const uint32_t t_s = tmem_s0 + b * 128 + lane_off;
-            // pass A: row max
-            float mx = -INFINITY;
-            uint32_t v[32];
-#pragma unroll 1
-            for (int c = 0; c < 4; ++c) {
-                tmem_ld32(t_s + c * 32, v);
-                tmem_ld_wait();
-#pragma unroll
-                for (int i = 0; i < 32; ++i) {
-                    float sv = __uint_as_float(v[i]);
-                    if (tail && kbase + c * 32 + i >= klim) sv = -INFINITY;
-                    mx = fmaxf(mx, sv);
-                }
-            }
-            const float m_new = fmaxf(m_run, mx * p.scale_log2);
-            const float alpha = exp2f(m_run - m_new);
-            m_run = m_new;
-            // P buffer must have been consumed by PV_{j-2}
-            mbar_wait(&p_empty[b], ((j >> 1) & 1) ^ 1);
-            uint8_t* p_row = smem + AttnSmem::OFF_P + b * AttnSmem::P_BYTES + r * 128;
-            float l_part = 0.f;
-            // pass B: probabilities
-#pragma unroll 1
-            for (int c = 0; c < 4; ++c) {
-                tmem_ld32(t_s + c * 32, v);
-                tmem_ld_wait();
-                uint32_t pk[16];
-#pragma unroll
-                for (int i = 0; i < 32; i += 2) {
-                    float p0 = exp2f(__uint_as_float(v[i]) * p.scale_log2 - m_new);
-                    float p1 = exp2f(__uint_as_float(v[i + 1]) * p.scale_log2 - m_new);
-                    if (tail) {
-                        if (kbase + c * 32 + i >= klim) p0 = 0.f;
-                        if (kbase + c * 32 + i + 1 >= klim) p1 = 0.f;
-                    }
-                    // the row sum uses the fp16-rounded probabilities that the PV MMA consumes
-                    __half2 h = __floats2half2_rn(p0, p1);
-                    float2 hf = __half22float2(h);
-                    l_part += hf.x + hf.y;
-                    pk[i >> 1] = *reinterpret_cast<uint32_t*>(&h);
-                }
-                // columns [c*32, c*32+32) -> 64-col block (c>>1), 16-byte chunks ((c&1)*4 .. +3), swizzled by row
-                uint8_t* blk = p_row + (c >> 1) * 16384;
-#pragma unroll
-                for (int u = 0; u < 4; ++u) {
-                    const int chunk = ((c & 1) * 4 + u) ^ (r & 7);
-                    *reinterpret_cast<uint4*>(blk + chunk * 16) = make_uint4(pk[u * 4], pk[u * 4 + 1], pk[u * 4 + 2], pk[u * 4 + 3]);
-                }
-            }
-            tc_fence_before();
-            mbar_arrive(&s_empty[b]);          // S[b] fully read
-            fence_proxy_async_smem();          // make P visible to the async (UMMA) proxy
-            mbar_arrive(&p_full[b]);
-            l_run = l_run * alpha + l_part;
-            if (j > 0) fold_o(j - 1);
-            alpha_prev = alpha;
-        }
-        fold_o(nt - 1);
-        const int q = q0 + r;
-        if (q < p.Nq) {
-            const float inv = 1.0f / l_run;
-            __half* op = p.out + ((long long)batch * p.Nq + q) * p.ldo + head * AT_D;
-#pragma unroll
-            for (int u = 0; u < 8; ++u) {
-                uint4 w;
-                w.x = pack_half2(o[u * 8 + 0] * inv, o[u * 8 + 1] * inv);
-                w.y = pack_half2(o[u * 8 + 2] * inv, o[u * 8 + 3] * inv);
-                w.z = pack_half2(o[u * 8 + 4] * inv, o[u * 8 + 5] * inv);
-                w.w = pack_half2(o[u * 8 + 6] * inv, o[u * 8 + 7] * inv);
-                reinterpret_cast<uint4*>(op)[u] = w;
-            }
-        }
+        return;
     }
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc<TMEM_COLS>(tmem_base);
+
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 240;");
+    const int cw = wg - 1;
+    const int q4 = lane & 3;
+    const int row_in_wg = (warp & 3) * 16 + (lane >> 2);
+    const int qrow[2] = {q0 + cw * 64 + row_in_wg, q0 + cw * 64 + row_in_wg + 8};
+    const uint64_t dq = wgmma_desc_sw128(smem_u32(smem + AttnSmem::OFF_Q) + cw * 64 * 128, 16, 1024);
+    const uint64_t dk0 = wgmma_desc_sw128(smem_u32(smem + AttnSmem::OFF_K), 16, 1024);
+    const uint64_t dv0 = wgmma_desc_sw128(smem_u32(smem + AttnSmem::OFF_V), 8192, 1024);
+    constexpr uint64_t TILE_INC = (uint64_t)(AttnSmem::TILE >> 4);
+    const float sl2 = p.scale_log2;
+
+    float o[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) o[i] = 0.f;
+    float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+
+    mbar_wait(q_full, 0);
+    int s = 0;
+    uint32_t ph = 0;
+#pragma unroll 1
+    for (int j = 0; j < nt; ++j) {
+        mbar_wait(&kv_full[s], ph);
+        float sacc[64];
+#pragma unroll
+        for (int i = 0; i < 64; ++i) sacc[i] = 0.f;
+        const uint64_t dk = dk0 + TILE_INC * (uint64_t)s;
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < AT_D / 16; ++k) wgmma_m64n128_ss(sacc, dq + 2 * k, dk + 2 * k);
+        wgmma_commit();
+        wgmma_wait<0>();
+
+        const int kbase = j * AT_BKV;
+        float alpha[2];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int klim = p.causal ? min(p.Nk, qrow[h] + 1) : p.Nk;     // keys [0, klim) are visible to this row
+            float mx = -INFINITY;
+            if (kbase + AT_BKV > klim) {
+#pragma unroll
+                for (int jj = 0; jj < 16; ++jj)
+#pragma unroll
+                    for (int e = 0; e < 2; ++e)
+                        if (kbase + 8 * jj + 2 * q4 + e >= klim) sacc[4 * jj + 2 * h + e] = -INFINITY;
+            }
+#pragma unroll
+            for (int jj = 0; jj < 16; ++jj) mx = fmaxf(mx, fmaxf(sacc[4 * jj + 2 * h], sacc[4 * jj + 2 * h + 1]));
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+            const float m_new = fmaxf(m_run[h], mx * sl2);
+            alpha[h] = ex2_approx(m_run[h] - m_new);
+            m_run[h] = m_new;
+            float l = 0.f;
+#pragma unroll
+            for (int jj = 0; jj < 16; ++jj)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const float pv = ex2_approx(fmaf(sacc[4 * jj + 2 * h + e], sl2, -m_new));
+                    sacc[4 * jj + 2 * h + e] = pv;
+                    l += pv;
+                }
+            l_run[h] = l_run[h] * alpha[h] + l;
+        }
+        // P as the A operand of P V: k-step kk covers keys [16 kk, 16 kk + 16) = accumulator columns of pairs 2kk, 2kk+1
+        uint32_t pa[AT_BKV / 16][4];
+#pragma unroll
+        for (int kk = 0; kk < AT_BKV / 16; ++kk) {
+            pa[kk][0] = pack_half2(sacc[8 * kk + 0], sacc[8 * kk + 1]);
+            pa[kk][1] = pack_half2(sacc[8 * kk + 2], sacc[8 * kk + 3]);
+            pa[kk][2] = pack_half2(sacc[8 * kk + 4], sacc[8 * kk + 5]);
+            pa[kk][3] = pack_half2(sacc[8 * kk + 6], sacc[8 * kk + 7]);
+        }
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) {
+            o[4 * jj + 0] *= alpha[0];
+            o[4 * jj + 1] *= alpha[0];
+            o[4 * jj + 2] *= alpha[1];
+            o[4 * jj + 3] *= alpha[1];
+        }
+        const uint64_t dv = dv0 + TILE_INC * (uint64_t)s;
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < AT_BKV / 16; ++kk) wgmma_m64n64_rs_tb(o, pa[kk], dv + (uint64_t)(kk * (2048 >> 4)));
+        wgmma_commit();
+        wgmma_wait<0>();
+        if (lane == 0) mbar_arrive(&kv_empty[s]);
+        if (++s == AT_KV_STAGES) { s = 0; ph ^= 1; }
+    }
+
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        float l = l_run[h];
+        l += __shfl_xor_sync(0xffffffffu, l, 1);
+        l += __shfl_xor_sync(0xffffffffu, l, 2);
+        const float inv = 1.0f / l;
+        if (qrow[h] < p.Nq) {
+            __half* op = p.out + ((long long)batch * p.Nq + qrow[h]) * p.ldo + head * AT_D + 2 * q4;
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj)
+                *reinterpret_cast<uint32_t*>(op + 8 * jj) = pack_half2(o[4 * jj + 2 * h] * inv, o[4 * jj + 2 * h + 1] * inv);
+        }
     }
 }
 

@@ -290,8 +290,8 @@ gn_stats2_kernel(const __half* __restrict__ x, double* __restrict__ stats, long 
         if (active) {
             const __half* xs = x + (sample * rows_per_sample) * C + oc * 8;
             long long r = r0 + ln;
-            for (; r + 3ll * lanes < r1; r += 4ll * lanes) {          // 4 independent 16-byte loads in flight (8 measured slower:
-                uint4 u[4];                                            // profiles/r02_kbench_gn_loads_ab.log)
+            for (; r + 3ll * lanes < r1; r += 4ll * lanes) {          // 4 independent 16-byte loads in flight
+                uint4 u[4];
 #pragma unroll
                 for (int k = 0; k < 4; ++k) u[k] = __ldg(reinterpret_cast<const uint4*>(xs + (r + (long long)k * lanes) * C));
 #pragma unroll
@@ -548,8 +548,7 @@ layernorm_kernel(const __half* __restrict__ x, const __half* __restrict__ gamma,
 
 // Narrow rows: C = 40 * LPR channels (320 -> LPR 8, 640 -> LPR 16).  A warp normalises 32 / LPR rows at once, LPR lanes
 // x 5 sixteen-byte groups per row, every lane busy (layernorm_kernel<2> keeps only 20 of 32 lanes busy at C = 320 and
-// spends a full 5-step shuffle tree per row: ~150 instructions per row against ~80 here; see
-// profiles/r01_kbench_rowops_v2.log).  Same arithmetic and gate modes as layernorm_kernel.
+// spends a full 5-step shuffle tree per row: ~150 instructions per row against ~80 here).  Same arithmetic and gate modes as layernorm_kernel.
 template <int LPR>
 __global__ void __launch_bounds__(256, 2)
 layernorm_sub_kernel(const __half* __restrict__ x, const __half* __restrict__ gamma, const __half* __restrict__ beta,

@@ -1,4 +1,4 @@
-// star_b200 / csrc / star_abi.cu -- host side of libstar_sm100.so (C ABI in include/star_sm100.h)
+// star_b200 / csrc / star_abi.cu -- host side of libstar_sm100.so, the sm_90a kernel library (C ABI in include/star_sm100.h)
 #include <cuda.h>
 #include <cudaTypedefs.h>
 #include <cuda_runtime.h>
@@ -13,11 +13,9 @@
 
 #include "../../include/star_sm100.h"
 #include "attn.cuh"
-#include "attn4.cuh"
 #include "rowops.cuh"
 #include "tattn2.cuh"
 #include "tapgemm.cuh"
-#include "tapgemm2.cuh"
 
 using namespace star;
 
@@ -27,20 +25,13 @@ thread_local std::string g_err;
 PFN_cuTensorMapEncodeTiled_v12000 g_encode = nullptr;
 constexpr int STAR_MAX_DEVICES = 64;
 int g_sms[STAR_MAX_DEVICES] = {0};            // SM count per initialised device (0 = star_init not called for it)
-// Tile-shape rules of the tap-GEMM dispatch (measured: profiles/r01_kbench_wide_tiles.log); constants, not switches.
-constexpr int kWideWastePct = 10;             // largest padding (percent of N) accepted for the 128x256 tiles ...
-constexpr int kWideWasteLongKPct = 25;        // ... and for reductions >= 1920 (N = 640 as 3 x 256: +16 % on the 640-channel convs)
-constexpr int kWideMinK = 256;                // smallest reduction length that takes the 128x256 tiles
-#ifndef STAR_GEMM_DBUF_MAXK
-#define STAR_GEMM_DBUF_MAXK 700               // 128x256-tile GEMMs with reductions up to this length use two output staging buffers
-#endif                                        // (A/B: profiles/r02_kbench_gemm_dbuf_ab.log -- qkv -5 %, 512->1536 -9 %, longer K / narrower tiles lose)
 std::atomic<long long> g_launches{0};
 
 // SM count of the CURRENT device (kernels are launched on the caller's current device / stream)
 inline int num_sms() {
     int dev = 0;
     if (cudaGetDevice(&dev) == cudaSuccess && dev >= 0 && dev < STAR_MAX_DEVICES && g_sms[dev] > 0) return g_sms[dev];
-    return 148;
+    return 132;
 }
 
 int fail(const char* fmt, ...) {
@@ -141,13 +132,16 @@ int launch_tapgemm_bn(const TapDesc& d, cudaStream_t st) {
     p.rowvec_div = (int)std::max(1ll, d.rowvec_div);
     p.rowvec_ld = d.ldrowvec > 0 ? d.ldrowvec : d.N;
     p.residual = (const __half*)d.residual;
+    p.colscale = (const __half*)d.colscale;
     p.res_ld = d.ldres;
     p.out = (__half*)d.out;
     p.out_ld = d.ldo;
     const bool geglu = d.flags & TG_GEGLU;
-    if (geglu && BN != 128) return fail("tapgemm: GEGLU requires BN=128");
-    if (geglu && (d.N % 64)) return fail("tapgemm: GEGLU requires N %% 64 == 0 (N=%d)", d.N);
-    if (m_tiles > 65535) return fail("tapgemm: %lld M tiles exceed grid.y", m_tiles);
+    const int n_per_tile = geglu ? BN / 2 : BN;
+    p.n_tiles = (d.N + n_per_tile - 1) / n_per_tile;
+    const long long total = m_tiles * p.n_tiles;
+    if (total > 0x7fffffffll) return fail("tapgemm: too many tiles");
+    p.num_tiles = (int)total;
 
     CUtensorMap ta, tw;
     unsigned abox[5] = {TG_BK, (unsigned)d.box[0], (unsigned)d.box[1], (unsigned)d.box[2], (unsigned)d.box[3]};
@@ -155,136 +149,25 @@ int launch_tapgemm_bn(const TapDesc& d, cudaStream_t st) {
     const unsigned long long wrows = geglu ? 2ull * d.N : (unsigned long long)d.N;
     unsigned long long wdim[2] = {(unsigned long long)d.ntaps * d.K, wrows};
     unsigned long long wstr[2] = {1, (unsigned long long)d.ntaps * d.K};
-    unsigned wbox[2] = {TG_BK, (unsigned)(geglu ? BN / 2 : BN)};
+    unsigned wbox[2] = {TG_BK, (unsigned)n_per_tile};
     if (make_tmap(&tw, d.W, 2, wdim, wstr, wbox)) return 1;
 
-    const int n_per_tile = geglu ? BN / 2 : BN;
-    dim3 grid((d.N + n_per_tile - 1) / n_per_tile, (unsigned)m_tiles, 1);
+    const int grid = (int)std::min<long long>(total, num_sms());
     tapgemm_kernel<BN><<<grid, TG_THREADS, TapGemmSmem<BN>::TOTAL, st>>>(ta, tw, p);
     STAR_LAUNCH_CHECK("tapgemm");
     return 0;
 }
 
-template <int BN>
-int launch_tapgemm2_bn(const TapDesc& d, cudaStream_t st) {
-    TapGemmParams p;
-    memset(&p, 0, sizeof(p));
-    long long m_tiles = 1;
-    int box_rows = 1;
-    for (int i = 0; i < 4; ++i) {
-        p.on[i] = d.on[i];
-        p.box[i] = d.box[i];
-        p.tiles[i] = (d.on[i] + d.box[i] - 1) / d.box[i];
-        m_tiles *= p.tiles[i];
-        box_rows *= d.box[i];
-    }
-    if (box_rows > TG_BM) return fail("tapgemm2: box has %d rows (> %d)", box_rows, TG_BM);
-    p.box_rows = box_rows;
-    p.ntaps = d.ntaps;
-    memcpy(p.tap, d.tap, sizeof(p.tap));
-    p.K = d.K;
-    p.k_chunks = (d.K + TG_BK - 1) / TG_BK;
-    p.N = d.N;
-    p.flags = d.flags;
-    p.bias = (const __half*)d.bias;
-    p.rowvec = (const __half*)d.rowvec;
-    p.rowvec_div = (int)std::max(1ll, d.rowvec_div);
-    p.rowvec_ld = d.ldrowvec > 0 ? d.ldrowvec : d.N;
-    p.residual = (const __half*)d.residual;
-    p.colscale = (const __half*)d.colscale;
-    p.res_ld = d.ldres;
-    p.out = (__half*)d.out;
-    p.out_ld = d.ldo;
-    const bool geglu = d.flags & TG_GEGLU;
-    const int n_per_tile = geglu ? BN / 2 : BN;
-    TapGemm2Extra ex;
-    ex.n_tiles = (d.N + n_per_tile - 1) / n_per_tile;
-    const long long total = m_tiles * ex.n_tiles;
-    if (total > 0x7fffffffll) return fail("tapgemm2: too many tiles");
-    ex.num_tiles = (int)total;
-
-    CUtensorMap ta, tw, to, tr;
-    unsigned abox[5] = {TG_BK, (unsigned)d.box[0], (unsigned)d.box[1], (unsigned)d.box[2], (unsigned)d.box[3]};
-    if (make_tmap(&ta, d.A, 5, d.adim, d.astr, abox)) return 1;
-    const unsigned long long wrows = geglu ? 2ull * d.N : (unsigned long long)d.N;
-    unsigned long long wdim[2] = {(unsigned long long)d.ntaps * d.K, wrows};
-    unsigned long long wstr[2] = {1, (unsigned long long)d.ntaps * d.K};
-    unsigned wbox[2] = {TG_BK, (unsigned)(geglu ? BN / 2 : BN)};
-    if (make_tmap(&tw, d.W, 2, wdim, wstr, wbox)) return 1;
-    // output / residual: (N, n1..n4) with row pitch ld; 32-column boxes, SWIZZLE_64B staging tiles
-    unsigned obox[5] = {32, (unsigned)d.box[0], (unsigned)d.box[1], (unsigned)d.box[2], (unsigned)d.box[3]};
-    unsigned long long odim[5] = {(unsigned long long)d.N, (unsigned long long)d.on[0], (unsigned long long)d.on[1],
-                                  (unsigned long long)d.on[2], (unsigned long long)d.on[3]};
-    auto strides = [&](long long ld, unsigned long long* s) {
-        s[0] = 1;
-        s[1] = (unsigned long long)ld;
-        s[2] = s[1] * d.on[0];
-        s[3] = s[2] * d.on[1];
-        s[4] = s[3] * d.on[2];
-    };
-    unsigned long long ostr[5], rstr[5];
-    strides(d.ldo, ostr);
-    if (make_tmap(&to, d.out, 5, odim, ostr, obox, CU_TENSOR_MAP_SWIZZLE_64B)) return 1;
-    // Output staging depth.  Short reductions are epilogue-bound (the main loop alone runs at 75-82 % of peak, the serialised
-    // store drain costs 25-30 %: profiles/r02_kbench_gemm_attribution.log) -> two staging buffers, one operand stage fewer.
-    ex.dbuf = ((long long)d.ntaps * d.K <= STAR_GEMM_DBUF_MAXK) ? 1 : 0;
-    ex.res_direct = 0;
-    const bool res_tma = d.residual && TapGemm2Smem<BN>::RES_TMA;
-    if (ex.dbuf && TapGemm2Smem<BN>::stages(res_tma, true) < 3) ex.dbuf = 0;       // BN = 160 + residual: no room for a second buffer
-    if (res_tma) {
-        strides(d.ldres, rstr);
-        if (make_tmap(&tr, d.residual, 5, odim, rstr, obox, CU_TENSOR_MAP_SWIZZLE_64B)) return 1;
-    } else {
-        tr = to;
-    }
-    const int grid = (int)std::min<long long>(total, num_sms());
-    ex.stages = TapGemm2Smem<BN>::stages(res_tma, ex.dbuf != 0);
-    const size_t smem = TapGemm2Smem<BN>::total(res_tma, ex.dbuf != 0);
-    // compile-time specialised epilogues for the three shapes that carry ~all of the linear / conv time
-    const bool extras = d.rowvec || d.colscale || (d.flags & (TG_GELU_TANH | TG_GELU_ERF | TG_SILU_OUT));
-    bool launched = false;
-    if (geglu && !d.residual && !extras) {
-        if constexpr (BN != 160) {
-            tapgemm2_kernel<BN, TG2_EPI_GEGLU><<<grid, TG2_THREADS, smem, st>>>(ta, tw, to, tr, p, ex);
-            launched = true;
-        }
-    } else if (!geglu && !d.residual && !extras) {
-        tapgemm2_kernel<BN, TG2_EPI_PLAIN><<<grid, TG2_THREADS, smem, st>>>(ta, tw, to, tr, p, ex);
-        launched = true;
-    } else if (!geglu && res_tma && !extras) {
-        if constexpr (TapGemm2Smem<BN>::RES_TMA) {
-            tapgemm2_kernel<BN, TG2_EPI_RES><<<grid, TG2_THREADS, smem, st>>>(ta, tw, to, tr, p, ex);
-            launched = true;
-        }
-    }
-    if (!launched) tapgemm2_kernel<BN, TG2_EPI_GENERIC><<<grid, TG2_THREADS, smem, st>>>(ta, tw, to, tr, p, ex);
-    STAR_LAUNCH_CHECK("tapgemm2");
-    return 0;
-}
-
+// Tile width: the one of 128 / 160 / 256 output columns (GEGLU: 64 / 128 value columns) that pads N least, the wider on
+// a tie (fewer tiles, more reuse of each A tile).
 int launch_tapgemm(const TapDesc& d, cudaStream_t st) {
     const bool geglu = d.flags & TG_GEGLU;
-    const bool aligned = (d.N % 32 == 0) && (d.ldo % 8 == 0) && (reinterpret_cast<uintptr_t>(d.out) % 16 == 0) &&
-                         (!d.residual || ((d.ldres % 8 == 0) && (reinterpret_cast<uintptr_t>(d.residual) % 16 == 0))) &&
-                         (!geglu || d.N % 64 == 0);
-    // Non-persistent kernel (2 CTAs/SM, two interleaved MMA streams) is measurably faster for the long-reduction,
-    // wide-N convolutions (profiles/r01_kbench_ab_experiments.txt); the persistent one wins everywhere else.
-    const bool v2_only = d.colscale != nullptr || (d.flags & (TG_GELU_TANH | TG_GELU_ERF));
-    if (v2_only && !aligned) return fail("tapgemm: colscale / GELU epilogues need N %% 32 == 0 and 16-byte aligned rows");
-    const bool long_k = ((long long)d.ntaps * d.K >= 3840) && (d.N % 128 == 0) && !geglu && !v2_only;
-    // 128x256 tiles (4 x 48 KB stages, two-pass epilogue): 25 % less L2->SM operand traffic per flop and N = 256 MMAs
-    // (137 clk per instruction against a 128 clk floor; N = 128 retires at 73 against 64: profiles/r01_micro_mma_rate.log)
-    // Used when the padded width wastes <= 10 % (<= 25 % for long reductions, where the tile-shape gain outweighs it:
-    // profiles/r01_kbench_wide_tiles.log) (N = 960, 1280, 1920, 2560, 3840, ...; GEGLU: 128 outputs per tile).
-    const int wide_n = geglu ? 128 : 256;
-    const long long padded = ((long long)d.N + wide_n - 1) / wide_n * wide_n;
-    const long long red = (long long)d.ntaps * d.K;
-    const bool wide = aligned && red >= kWideMinK &&
-                      padded * 100 <= (long long)d.N * (100 + (red >= 1920 ? kWideWasteLongKPct : kWideWastePct));
-    if (wide) return launch_tapgemm2_bn<256>(d, st);
-    const bool n160 = !geglu && d.N % 160 == 0 && d.N % 128 != 0;
-    if (aligned && !long_k) return n160 ? launch_tapgemm2_bn<160>(d, st) : launch_tapgemm2_bn<128>(d, st);
-    return n160 ? launch_tapgemm_bn<160>(d, st) : launch_tapgemm_bn<128>(d, st);
+    auto padded = [&](int w) { return ((long long)d.N + w - 1) / w * w; };
+    if (geglu) return padded(128) <= padded(64) ? launch_tapgemm_bn<256>(d, st) : launch_tapgemm_bn<128>(d, st);
+    const long long p128 = padded(128), p160 = padded(160), p256 = padded(256);
+    if (p256 <= p128 && p256 <= p160) return launch_tapgemm_bn<256>(d, st);
+    if (p160 <= p128) return launch_tapgemm_bn<160>(d, st);
+    return launch_tapgemm_bn<128>(d, st);
 }
 
 void best_box_2d(int H, int W, int* th, int* tw) {
@@ -318,7 +201,7 @@ long long star_launch_count(void) { return g_launches.load(); }
 static int star_init_on_current(int device) {
     cudaDeviceProp prop;
     STAR_CUDA(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10) return fail("libstar_sm100 needs an sm_100 device, found sm_%d%d", prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0) return fail("libstar_sm100 is built for sm_90a and needs an sm_90 device, found sm_%d%d", prop.major, prop.minor);
     if (!g_encode) {
         void* fn = nullptr;
         cudaDriverEntryPointQueryResult qr;
@@ -329,19 +212,8 @@ static int star_init_on_current(int device) {
 #define STAR_SMEM_ATTR(kernel, bytes) STAR_CUDA((cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(bytes))))
     STAR_SMEM_ATTR(tapgemm_kernel<128>, TapGemmSmem<128>::TOTAL);
     STAR_SMEM_ATTR(tapgemm_kernel<160>, TapGemmSmem<160>::TOTAL);
-    STAR_SMEM_ATTR((tapgemm2_kernel<128, TG2_EPI_GENERIC>), 232448);
-    STAR_SMEM_ATTR((tapgemm2_kernel<160, TG2_EPI_GENERIC>), 232448);
-    STAR_SMEM_ATTR((tapgemm2_kernel<256, TG2_EPI_GENERIC>), 232448);
-    STAR_SMEM_ATTR((tapgemm2_kernel<128, TG2_EPI_PLAIN>), 232448);
-    STAR_SMEM_ATTR((tapgemm2_kernel<160, TG2_EPI_PLAIN>), 232448);
-    STAR_SMEM_ATTR((tapgemm2_kernel<256, TG2_EPI_PLAIN>), 232448);
-    STAR_SMEM_ATTR((tapgemm2_kernel<128, TG2_EPI_RES>), 232448);
-    STAR_SMEM_ATTR((tapgemm2_kernel<160, TG2_EPI_RES>), 232448);
-    STAR_SMEM_ATTR((tapgemm2_kernel<128, TG2_EPI_GEGLU>), 232448);
-    STAR_SMEM_ATTR((tapgemm2_kernel<256, TG2_EPI_GEGLU>), 232448);
-    STAR_SMEM_ATTR(attn_fwd_kernel<false>, AttnSmemT<false>::TOTAL);
-    STAR_SMEM_ATTR(attn_fwd_kernel<true>, AttnSmemT<true>::TOTAL);
-    STAR_SMEM_ATTR(attn4_fwd_kernel, Attn4Smem::TOTAL);
+    STAR_SMEM_ATTR(tapgemm_kernel<256>, TapGemmSmem<256>::TOTAL);
+    STAR_SMEM_ATTR(attn_fwd_kernel, AttnSmem::TOTAL);
     STAR_SMEM_ATTR(temporal_attn2_kernel<16>, TA2_WARPS * 3 * 16 * TA2_PITCH);
     STAR_SMEM_ATTR(temporal_attn2_kernel<32>, TA2_WARPS * 3 * 32 * TA2_PITCH);
     STAR_SMEM_ATTR(temporal_attn2_kernel<48>, TA2_WARPS * 3 * 48 * TA2_PITCH);
@@ -566,19 +438,8 @@ static int attention_impl(const void* Q, long long ldq, const void* K, long long
     p.scale_log2 = scale * 1.4426950408889634f;
     p.out = (__half*)O; p.ldo = ldo;
     if (heads > 65535 || batch > 65535) return fail("star_attention: grid too large");
-    cudaStream_t st = (cudaStream_t)stream;
-    // Multi-tile problems (spatial self-attention): two 128-row query tiles per CTA, row-split softmax, every exponential on
-    // the MUFU (in-step A/B on the full model: profiles/r01_bench_ab_attention.log).  Single-KV-tile problems (text
-    // cross-attention, tiny latents): the one-tile kernel, two CTAs per SM.
-    if (Nk > AT_BKV && Nq > AT_BQ && !causal) {
-        dim3 grid((Nq + 255) / 256, heads, batch);
-        attn4_fwd_kernel<<<grid, A4S_THREADS, Attn4Smem::TOTAL, st>>>(tq, tk, tv, p);
-        STAR_LAUNCH_CHECK("attn4_fwd");
-        return 0;
-    }
     dim3 grid((Nq + AT_BQ - 1) / AT_BQ, heads, batch);
-    if (Nk <= AT_BKV) attn_fwd_kernel<true><<<grid, AT_THREADS, AttnSmemT<true>::TOTAL, st>>>(tq, tk, tv, p);
-    else attn_fwd_kernel<false><<<grid, AT_THREADS, AttnSmemT<false>::TOTAL, st>>>(tq, tk, tv, p);
+    attn_fwd_kernel<<<grid, AT_THREADS, AttnSmem::TOTAL, (cudaStream_t)stream>>>(tq, tk, tv, p);
     STAR_LAUNCH_CHECK("attn_fwd");
     return 0;
 }
@@ -899,30 +760,6 @@ int star_cfg_x0(const void* y_out, const void* u_out, const void* xt_f32, void* 
     STAR_LAUNCH_CHECK("cfg_x0");
     return 0;
 }
-
-#if STAR_GEMM_TRACE
-// experiment builds only (tools/gemm_trace.py): copy CTA 0's role timelines to the host and reset them
-int star_debug_read_trace(long long* host_dst, int* host_counts) {
-    STAR_CUDA(cudaDeviceSynchronize());
-    STAR_CUDA(cudaMemcpyFromSymbol(host_dst, g_tg2_trace, sizeof(long long) * 3 * 4096));
-    STAR_CUDA(cudaMemcpyFromSymbol(host_counts, g_tg2_trace_n, sizeof(int) * 3));
-    int zero[3] = {0, 0, 0};
-    STAR_CUDA(cudaMemcpyToSymbol(g_tg2_trace_n, zero, sizeof(zero)));
-    return 0;
-}
-#endif
-
-#if STAR_ATTN_TRACE
-// experiment builds only (tools/attn_trace.py): softmax-phase timelines of CTA (0,0,0) of the spatial-attention kernel
-int star_debug_read_attn_trace(long long* host_dst, int* host_counts) {
-    STAR_CUDA(cudaDeviceSynchronize());
-    STAR_CUDA(cudaMemcpyFromSymbol(host_dst, g_a4_trace, sizeof(long long) * 2 * 8192));
-    STAR_CUDA(cudaMemcpyFromSymbol(host_counts, g_a4_trace_n, sizeof(int) * 2));
-    int zero[2] = {0, 0};
-    STAR_CUDA(cudaMemcpyToSymbol(g_a4_trace_n, zero, sizeof(zero)));
-    return 0;
-}
-#endif
 
 int star_sinusoidal(const void* t_i64, void* out, int B, int dim, void* stream) {
     const int n = B * (dim / 2);

@@ -1,5 +1,5 @@
 // star_b200 / csrc / tapgemm.cuh
-// "tap-GEMM": one tcgen05 implicit-GEMM kernel for every dense contraction of the
+// "tap-GEMM": one wgmma implicit-GEMM kernel for every dense contraction of the
 // STAR UNet on channels-last fp16 activations:
 //     Out[row, n] = epi( sum_{tap} sum_{k} A[row + tap_offset, k] * W[n, tap*K + k] )
 //   * Linear / 1x1 conv / Conv1d(k=1)   : 1 tap                 (unet_v2v.py:151-155, :274, :1005)
@@ -13,20 +13,22 @@
 // coordinates are zero-filled by TMA, which implements the conv zero padding and the
 // ragged tile edges with no im2col buffer and no extra HBM traffic.
 //
-// Warp roles (192 threads): warp 0 = TMA producer, warp 1 = TMEM owner + single-thread
-// tcgen05.mma issuer, warps 2..5 = epilogue (TMEM -> registers -> fused epilogue -> HBM).
-// Two CTAs are resident per SM (3 smem stages each) so one CTA's epilogue overlaps the
-// other's main loop.
+// Persistent kernel, one CTA per SM looping over 128 x BN output tiles (n fastest, so concurrently running CTAs
+// share the A tile in L2).  Warpgroup 0: one TMA producer thread filling a ring of (A, W) stages; warpgroups 1 and 2:
+// consumers, each computing 64 tile rows x BN columns with wgmma (fp32 accumulators in registers) and applying the
+// fused epilogue straight from registers.  The producer runs ahead into the next tile while the consumers finish the
+// epilogue of the current one.
 #pragma once
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace star {
 
-constexpr int TG_BM = 128;      // rows (pixels) per tile == TMEM lanes
+constexpr int TG_BM = 128;      // rows (pixels) per tile
 constexpr int TG_BK = 64;       // fp16 K elements per stage == 128 B swizzle span
-constexpr int TG_STAGES = 3;
 constexpr int TG_MAX_TAPS = 27;   // 3x3x3 causal Conv3d of the CogVideoX VAE (cp_enc_dec.py:360-430)
-constexpr int TG_THREADS = 192;
+constexpr int TG_THREADS = 384;
+constexpr int TG_CONSUMER_WARPS = 8;
 
 enum TapGemmFlags : int {
     TG_GEGLU = 1,        // W has 2N rows (value | gate); out = value * gelu_erf(gate)
@@ -46,6 +48,8 @@ struct TapGemmParams {
     int k_chunks;         // ceil(K / 64)
     int N;                // output columns
     int flags;
+    int num_tiles;        // m_tiles * n_tiles
+    int n_tiles;
     const __half* bias;   // [N] ([2N] with GEGLU) or null
     const __half* rowvec; // [rows_out / rowvec_div, N] or null  (time-embedding add, unet_v2v.py:684)
     int rowvec_div;
@@ -62,219 +66,199 @@ struct TapGemmSmem {
     static constexpr int A_BYTES = TG_BM * TG_BK * 2;          // 16 KB
     static constexpr int B_BYTES = BN * TG_BK * 2;
     static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-    static constexpr int TOTAL = TG_STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+    static constexpr int MAX_STAGES = 8;
+    static constexpr int STAGES_FIT = (232448 - 1024 - 256) / STAGE_BYTES;     // 227 KB minus alignment slack and barriers
+    static constexpr int STAGES = STAGES_FIT < MAX_STAGES ? STAGES_FIT : MAX_STAGES;
+    static constexpr int TOTAL = STAGES * STAGE_BYTES + 1024 + 256;
 };
 
 template <int BN>
-__global__ void __launch_bounds__(TG_THREADS, 2)
+STAR_DEVINL void tg_mma_k16(float* acc, uint64_t da, uint64_t db) {
+    if constexpr (BN == 128) wgmma_m64n128_ss(acc, da, db);
+    else if constexpr (BN == 160) wgmma_m64n160_ss(acc, da, db);
+    else wgmma_m64n256_ss(acc, da, db);
+}
+
+STAR_DEVINL float tg_ld(const __half* p) { return __half2float(__ldg(p)); }
+
+template <int BN>
+__global__ void __launch_bounds__(TG_THREADS, 1)
 tapgemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_w,
                const __grid_constant__ TapGemmParams p) {
     using SM = TapGemmSmem<BN>;
-    constexpr uint32_t TMEM_COLS = (BN <= 128) ? 128 : 256;
+    constexpr int NS = SM::STAGES;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + TG_STAGES * SM::STAGE_BYTES);
-    uint64_t* empty_bar = full_bar + TG_STAGES;
-    uint64_t* acc_bar = empty_bar + TG_STAGES;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_bar + 1);
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + NS * SM::STAGE_BYTES);
+    uint64_t* empty_bar = full_bar + NS;
 
+    const int wg = threadIdx.x >> 7;
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
     const bool geglu = (p.flags & TG_GEGLU) != 0;
-    const int n_per_tile = geglu ? BN / 2 : BN;      // output columns produced per CTA
-    const int n_tile = blockIdx.x;
-    int m_tile = blockIdx.y;
-    int org[4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-        org[i] = (m_tile % p.tiles[i]) * p.box[i];
-        m_tile /= p.tiles[i];
-    }
+    const int n_per_tile = geglu ? BN / 2 : BN;      // output columns produced per tile
     const int total_iters = p.ntaps * p.k_chunks;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         tma_prefetch_desc(&tmap_a);
         tma_prefetch_desc(&tmap_w);
-    }
-    if (warp == 1) {
-        if (lane == 0) {
-            for (int s = 0; s < TG_STAGES; ++s) {
-                mbar_init(&full_bar[s], 1);
-                mbar_init(&empty_bar[s], 1);
-            }
-            mbar_init(acc_bar, 1);
-            fence_barrier_init();
+        for (int s = 0; s < NS; ++s) {
+            mbar_init(&full_bar[s], 1);
+            mbar_init(&empty_bar[s], TG_CONSUMER_WARPS);
         }
-        __syncwarp();
-        tmem_alloc<TMEM_COLS>(tmem_slot);
+        fence_barrier_init();
     }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_acc = *tmem_slot;
 
-    if (warp == 0) {
-        // ------------------------------------------------ TMA producer
-        if (lane == 0) {
-            const uint32_t tx = (uint32_t)p.box_rows * 128u + (uint32_t)SM::B_BYTES;
-            int it = 0;
-            for (int t = 0; t < p.ntaps; ++t) {
-                const int c1 = org[0] + p.tap[t][0], c2 = org[1] + p.tap[t][1];
-                const int c3 = org[2] + p.tap[t][2], c4 = org[3] + p.tap[t][3];
-                for (int kc = 0; kc < p.k_chunks; ++kc, ++it) {
-                    const int s = it % TG_STAGES;                 // compile-time modulus (3)
-                    const uint32_t ph = (it / TG_STAGES) & 1;
-                    mbar_wait(&empty_bar[s], ph ^ 1);
-                    uint8_t* sa = smem + s * SM::STAGE_BYTES;
-                    uint8_t* sb = sa + SM::A_BYTES;
-                    mbar_expect_tx(&full_bar[s], tx);
-                    tma_load_5d(sa, &tmap_a, &full_bar[s], kc * TG_BK, c1, c2, c3, c4);
-                    const int kw = t * p.K + kc * TG_BK;
-                    if (!geglu) {
-                        tma_load_2d(sb, &tmap_w, &full_bar[s], kw, n_tile * BN);
-                    } else {
-                        tma_load_2d(sb, &tmap_w, &full_bar[s], kw, n_tile * (BN / 2));
-                        tma_load_2d(sb + (BN / 2) * 128, &tmap_w, &full_bar[s], kw, p.N + n_tile * (BN / 2));
-                    }
-                }
-            }
-        }
-    } else if (warp == 1) {
-        // ------------------------------------------------ MMA issuer (one thread)
-        if (lane == 0) {
-            constexpr uint32_t idesc = umma_idesc_f16(TG_BM, BN, 0, 0);
-            const uint64_t desc_a0 = umma_desc_sw128(smem_u32(smem), 16, 1024);
-            const uint64_t desc_b0 = umma_desc_sw128(smem_u32(smem) + SM::A_BYTES, 16, 1024);
-            constexpr uint64_t STAGE_INC = (uint64_t)(SM::STAGE_BYTES >> 4);
-            int s = 0;
-            uint32_t ph = 0;
-            for (int it = 0; it < total_iters; ++it) {
-                mbar_wait(&full_bar[s], ph);
-                tc_fence_after();
-                const uint64_t da = desc_a0 + STAGE_INC * (uint64_t)s;
-                const uint64_t db = desc_b0 + STAGE_INC * (uint64_t)s;
-                umma_f16_ss(tmem_acc, da, db, idesc, it > 0 ? 1u : 0u);
-                umma_f16_ss(tmem_acc, da + 2, db + 2, idesc, 1u);
-                umma_f16_ss(tmem_acc, da + 4, db + 4, idesc, 1u);
-                umma_f16_ss(tmem_acc, da + 6, db + 6, idesc, 1u);
-                umma_commit(&empty_bar[s]);          // frees the smem stage when these MMAs retire
-                if (++s == TG_STAGES) { s = 0; ph ^= 1; }
-            }
-            umma_commit(acc_bar);                    // accumulator complete
-        }
-    } else {
-        // ------------------------------------------------ epilogue warps 2..5
-        const int q = warp & 3;                      // TMEM lane quadrant this warp may access
-        const int r = q * 32 + lane;                 // tile row == TMEM lane
-        // row -> output coordinates
-        int rr = r;
-        long long orow = 0, mul = 1;
-        bool valid = r < p.box_rows;
+    auto tile_origin = [&](int tile, int* org, int& n_tile) {
+        n_tile = tile % p.n_tiles;
+        int m_tile = tile / p.n_tiles;
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
-            const int l = rr % p.box[i];
-            rr /= p.box[i];
-            const int g = org[i] + l;
-            valid = valid && (g < p.on[i]);
-            orow += (long long)g * mul;
-            mul *= p.on[i];
+            org[i] = (m_tile % p.tiles[i]) * p.box[i];
+            m_tile /= p.tiles[i];
         }
-        const int n_base = n_tile * n_per_tile;
-        mbar_wait(acc_bar, 0);
-        tc_fence_after();
-        const uint32_t t_row = tmem_acc + ((uint32_t)(q * 32) << 16);
-        __half* out_row = p.out + orow * p.out_ld;
-        const __half* res_row = p.residual ? p.residual + orow * p.res_ld : nullptr;
-        const __half* rv_row = p.rowvec ? p.rowvec + (orow / p.rowvec_div) * p.rowvec_ld : nullptr;
-        const bool vec_ok = ((p.out_ld & 7) == 0) && ((reinterpret_cast<uintptr_t>(p.out) & 15) == 0) &&
-                            (!p.residual || (((p.res_ld & 7) == 0) && ((reinterpret_cast<uintptr_t>(p.residual) & 15) == 0)));
-#pragma unroll 1
-        for (int c0 = 0; c0 < n_per_tile; c0 += 32) {
-            uint32_t v[32];
-            float f[32];
-            tmem_ld32(t_row + c0, v);
-            if (geglu) {
-                uint32_t g[32];
-                tmem_ld32(t_row + (BN / 2) + c0, g);
-                tmem_ld_wait();
-#pragma unroll
-                for (int j = 0; j < 32; ++j) {
-                    const int n = n_base + c0 + j;
-                    float xv = __uint_as_float(v[j]), gv = __uint_as_float(g[j]);
-                    if (p.bias && n < p.N) {
-                        xv += __half2float(__ldg(p.bias + n));
-                        gv += __half2float(__ldg(p.bias + p.N + n));
-                    }
-                    f[j] = xv * gelu_erf_f(gv);
-                }
-            } else {
-                tmem_ld_wait();
-#pragma unroll
-                for (int j = 0; j < 32; ++j) {
-                    const int n = n_base + c0 + j;
-                    float xv = __uint_as_float(v[j]);
-                    if (p.bias && n < p.N) xv += __half2float(__ldg(p.bias + n));
-                    f[j] = xv;
-                }
-            }
-            const int n0 = n_base + c0;
-            const int ncols = min(32, min(n_per_tile - c0, p.N - n0));   // valid columns of this chunk
-            if (valid && ncols > 0) {
-                const bool full = (ncols == 32);
-                if (rv_row) {
-#pragma unroll
-                    for (int j = 0; j < 32; ++j)
-                        if (j < ncols) f[j] += __half2float(__ldg(rv_row + n0 + j));
-                }
-                if (res_row) {
-                    if (full && vec_ok) {
-                        const uint4* rp = reinterpret_cast<const uint4*>(res_row + n0);
-#pragma unroll
-                        for (int u = 0; u < 4; ++u) {
-                            uint4 t4 = __ldg(rp + u);
-                            const __half2* h2 = reinterpret_cast<const __half2*>(&t4);
-#pragma unroll
-                            for (int e = 0; e < 4; ++e) {
-                                float2 ff = __half22float2(h2[e]);
-                                f[u * 8 + e * 2] += ff.x;
-                                f[u * 8 + e * 2 + 1] += ff.y;
-                            }
+    };
+
+    if (wg == 0) {
+        // ------------------------------------------------ TMA producer
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+        if (threadIdx.x == 0) {
+            const uint32_t tx = (uint32_t)p.box_rows * 128u + (uint32_t)SM::B_BYTES;
+            int s = 0;
+            uint32_t ph = 0;
+            for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+                int org[4], n_tile;
+                tile_origin(tile, org, n_tile);
+                for (int t = 0; t < p.ntaps; ++t) {
+                    const int c1 = org[0] + p.tap[t][0], c2 = org[1] + p.tap[t][1];
+                    const int c3 = org[2] + p.tap[t][2], c4 = org[3] + p.tap[t][3];
+                    for (int kc = 0; kc < p.k_chunks; ++kc) {
+                        mbar_wait(&empty_bar[s], ph ^ 1);
+                        uint8_t* sa = smem + s * SM::STAGE_BYTES;
+                        uint8_t* sb = sa + SM::A_BYTES;
+                        mbar_expect_tx(&full_bar[s], tx);
+                        tma_load_5d(sa, &tmap_a, &full_bar[s], kc * TG_BK, c1, c2, c3, c4);
+                        const int kw = t * p.K + kc * TG_BK;
+                        if (!geglu) {
+                            tma_load_2d(sb, &tmap_w, &full_bar[s], kw, n_tile * BN);
+                        } else {
+                            tma_load_2d(sb, &tmap_w, &full_bar[s], kw, n_tile * (BN / 2));
+                            tma_load_2d(sb + (BN / 2) * 128, &tmap_w, &full_bar[s], kw, p.N + n_tile * (BN / 2));
                         }
-                    } else {
-#pragma unroll
-                        for (int j = 0; j < 32; ++j)
-                            if (j < ncols) f[j] += __half2float(res_row[n0 + j]);
+                        if (++s == NS) { s = 0; ph ^= 1; }
                     }
-                }
-                if (p.flags & TG_SILU_OUT) {
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) f[j] = silu_f(f[j]);
-                }
-                if (full && vec_ok) {
-                    uint4* op = reinterpret_cast<uint4*>(out_row + n0);
-#pragma unroll
-                    for (int u = 0; u < 4; ++u) {
-                        uint4 o;
-                        o.x = pack_half2(f[u * 8 + 0], f[u * 8 + 1]);
-                        o.y = pack_half2(f[u * 8 + 2], f[u * 8 + 3]);
-                        o.z = pack_half2(f[u * 8 + 4], f[u * 8 + 5]);
-                        o.w = pack_half2(f[u * 8 + 6], f[u * 8 + 7]);
-                        op[u] = o;
-                    }
-                } else {
-#pragma unroll
-                    for (int j = 0; j < 32; ++j)
-                        if (j < ncols) out_row[n0 + j] = __float2half_rn(f[j]);
                 }
             }
-            __syncwarp();
         }
-        tc_fence_before();
+        return;
     }
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc<TMEM_COLS>(tmem_acc);
+
+    // ---------------------------------------------------- consumers: warpgroup cw owns tile rows [64 cw, 64 cw + 64)
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    const int cw = wg - 1;
+    const int q4 = lane & 3;
+    const int row_in_wg = (warp & 3) * 16 + (lane >> 2);
+    const uint64_t desc_a0 = wgmma_desc_sw128(smem_u32(smem) + cw * 64 * 128, 16, 1024);
+    const uint64_t desc_b0 = wgmma_desc_sw128(smem_u32(smem) + SM::A_BYTES, 16, 1024);
+    constexpr uint64_t STAGE_INC = (uint64_t)(SM::STAGE_BYTES >> 4);
+    const bool has_bias = p.bias != nullptr, has_rowvec = p.rowvec != nullptr, has_colscale = p.colscale != nullptr;
+    const bool has_res = p.residual != nullptr;
+    const bool act_tanh = (p.flags & TG_GELU_TANH) != 0, act_erf = (p.flags & TG_GELU_ERF) != 0;
+    const bool act_silu = (p.flags & TG_SILU_OUT) != 0;
+    const bool out_pair = ((p.out_ld & 1) == 0) && ((reinterpret_cast<uintptr_t>(p.out) & 3) == 0);
+    const bool res_pair = !has_res || (((p.res_ld & 1) == 0) && ((reinterpret_cast<uintptr_t>(p.residual) & 3) == 0));
+    int s = 0;
+    uint32_t ph = 0;
+    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+        int org[4], n_tile;
+        tile_origin(tile, org, n_tile);
+        float acc[BN / 2];
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+        int prev_s = -1;
+#pragma unroll 1
+        for (int it = 0; it < total_iters; ++it) {
+            mbar_wait(&full_bar[s], ph);
+            const uint64_t da = desc_a0 + STAGE_INC * (uint64_t)s;
+            const uint64_t db = desc_b0 + STAGE_INC * (uint64_t)s;
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < TG_BK / 16; ++k) tg_mma_k16<BN>(acc, da + 2 * k, db + 2 * k);
+            wgmma_commit();
+            wgmma_wait<1>();                         // the MMAs of the previous stage have retired: release it
+            if (prev_s >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_s]);
+            prev_s = s;
+            if (++s == NS) { s = 0; ph ^= 1; }
+        }
+        wgmma_wait<0>();
+        if (prev_s >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_s]);
+
+        // ------------------------------------------------ epilogue: rows row_in_wg and row_in_wg + 8 of this warpgroup
+        const int n_base = n_tile * n_per_tile;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int r = cw * 64 + row_in_wg + 8 * h;
+            int rr = r;
+            long long orow = 0, mul = 1;
+            bool valid = r < p.box_rows;
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const int l = rr % p.box[i];
+                rr /= p.box[i];
+                const int g = org[i] + l;
+                valid = valid && (g < p.on[i]);
+                orow += (long long)g * mul;
+                mul *= p.on[i];
+            }
+            if (!valid) continue;
+            __half* out_row = p.out + orow * p.out_ld;
+            const __half* res_row = has_res ? p.residual + orow * p.res_ld : nullptr;
+            const __half* rv_row = has_rowvec ? p.rowvec + (orow / p.rowvec_div) * p.rowvec_ld : nullptr;
+#pragma unroll
+            for (int j = 0; j < BN / 8; ++j) {
+                if (geglu && j >= BN / 16) break;
+                const int c = 8 * j + 2 * q4;                    // tile column of this thread's pair
+                const int n = n_base + c;
+                if (c >= n_per_tile || n >= p.N) continue;
+                const bool two = n + 1 < p.N;
+                float f[2];
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    float x = acc[4 * j + 2 * h + e];
+                    const int ne = (e == 1 && !two) ? n : n + e;     // clamped index for the loads of a lone last column
+                    if (geglu) {
+                        float g = acc[4 * (j + BN / 16) + 2 * h + e];
+                        if (has_bias) { x += tg_ld(p.bias + ne); g += tg_ld(p.bias + p.N + ne); }
+                        x *= gelu_erf_f(g);
+                    } else if (has_bias) {
+                        x += tg_ld(p.bias + ne);
+                    }
+                    if (act_tanh) x = gelu_tanh_f(x);
+                    if (act_erf) x = gelu_erf_f(x);
+                    if (has_colscale) x *= tg_ld(p.colscale + ne);
+                    if (has_rowvec) x += tg_ld(rv_row + ne);
+                    f[e] = x;
+                }
+                if (has_res) {
+                    if (two && res_pair) {
+                        const float2 rv = __half22float2(*reinterpret_cast<const __half2*>(res_row + n));
+                        f[0] += rv.x;
+                        f[1] += rv.y;
+                    } else {
+                        f[0] += __half2float(res_row[n]);
+                        if (two) f[1] += __half2float(res_row[n + 1]);
+                    }
+                }
+                if (act_silu) { f[0] = silu_f(f[0]); f[1] = silu_f(f[1]); }
+                if (two && out_pair) {
+                    *reinterpret_cast<uint32_t*>(out_row + n) = pack_half2(f[0], f[1]);
+                } else {
+                    out_row[n] = __float2half_rn(f[0]);
+                    if (two) out_row[n + 1] = __float2half_rn(f[1]);
+                }
+            }
+        }
     }
 }
 

@@ -3,8 +3,8 @@
 // The problem is a 32x32x64 attention per item, 131 760 items per call at level 0: HBM-bound (the q|k|v
 // rows of a pixel are 128-byte segments strided by H*W rows).  v1 did the two small matmuls on the FMA
 // pipes with per-element fp16->fp32 converts and was instruction-bound (988 GB/s).  Here one warp handles
-// one item with warp-level tensor-core MMAs (mma.sync m16n8k16, fp16 in / fp32 accumulate): a 128x128
-// tcgen05 tile cannot be filled by a 32-row problem, and the kernel stays memory-bound either way.
+// one item with warp-level tensor-core MMAs (mma.sync m16n8k16, fp16 in / fp32 accumulate): a 64-row
+// wgmma tile cannot be filled by a 32-row problem, and the kernel stays memory-bound either way.
 //   * Q, K, V rows are copied global -> smem with 16-byte cp.async (4 rows per warp instruction), padded row
 //     pitch 144 B so ldmatrix is conflict-free; rows >= T are zero-filled and masked
 //   * per 16-query block: S = Q K^T in registers, row softmax with quad shuffles, P re-used as the A

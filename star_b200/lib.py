@@ -2,7 +2,7 @@
 
 The library is the only compute backend of star_b200: there is no CPU or
 PyTorch fallback.  ``get_lib()`` raises if the shared object is missing and
-``ensure_init()`` raises if no sm_100 device is available.
+``ensure_init()`` raises if no sm_90 (H100) device is available.
 """
 import ctypes
 import os
@@ -79,7 +79,7 @@ def get_lib(dtype=None):
         if not os.path.isfile(path):
             raise StarError(
                 f"{path} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-                "(nvcc, sm_100a). star_b200 has no fallback compute path.")
+                "(nvcc, sm_90a). star_b200 has no fallback compute path.")
         lib = ctypes.CDLL(path)
         for name, (res, args) in SIGNATURES.items():
             fn = getattr(lib, name)

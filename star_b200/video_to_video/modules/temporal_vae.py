@@ -1,4 +1,4 @@
-"""Temporal VAE (SVD `AutoencoderKLTemporalDecoder`) on the sm_100a kernels -- SURVEY rows a3 / a16.
+"""Temporal VAE (SVD `AutoencoderKLTemporalDecoder`) on the sm_90a kernels -- SURVEY rows a3 / a16.
 
 The reference builds this module from diffusers (video_to_video/video_to_video_model.py:57-63) and uses exactly
 three things of it (:141-161): ``vae.config.scaling_factor``, ``vae.encode(x).latent_dist.sample()`` per frame and
@@ -7,7 +7,7 @@ parameter tree (same keys and shapes as diffusers 0.30.0, so ``diffusion_pytorch
 ``load_state_dict``); ``nn`` only stores the parameters.  Execution keeps every activation as an fp16 token matrix
 X[(frame h w), C] and is a sequence of C-ABI calls (star_b200/ops.py):
 
-* all 3x3 / (3,1,1) / 1x1 convolutions -> tcgen05 implicit GEMM with bias + residual epilogues; the stride-2
+* all 3x3 / (3,1,1) / 1x1 convolutions -> wgmma implicit GEMM with bias + residual epilogues; the stride-2
   encoder convs (F.pad (0,1,0,1) + stride 2) through the parity-plane split; stems with Cin <= 4 through im2col;
 * GroupNorm(+SiLU) -> the two-pass GroupNorm kernels, per frame for the spatial blocks, per clip for the temporal ones;
 * AlphaBlender: out = a*x_s + (1-a)*(x_s + h) = x_s + sigmoid(mix_factor)*h, i.e. the second temporal conv with its

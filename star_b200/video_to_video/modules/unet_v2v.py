@@ -1,4 +1,4 @@
-"""STAR denoiser (3-D UNet + VideoControlNet with LIEM gates) on sm_100a kernels.
+"""STAR denoiser (3-D UNet + VideoControlNet with LIEM gates) on sm_90a kernels.
 
 Drop-in for the model surface of the reference's
 video_to_video/modules/unet_v2v.py: the classes below keep the reference's
@@ -9,9 +9,9 @@ for the default config, including the ``temopral_conv`` spelling, ref :651).
 Execution is completely different from the reference.  ``nn`` layers are only
 parameter containers; the forward pass keeps every activation as an fp16
 channels-last token matrix X[(b t h w), C] and is a sequence of calls into
-libstar_sm100.so (star_b200/ops.py): tcgen05 implicit-GEMM convolutions /
+libstar_sm100.so (star_b200/ops.py): wgmma implicit-GEMM convolutions /
 linears with fused bias + time-embedding + residual + GEGLU epilogues, a
-tcgen05 flash attention for the H*W-token spatial attention, a temporal
+wgmma flash attention for the H*W-token spatial attention, a temporal
 attention kernel over T, and 128-bit-vectorised GroupNorm / LayerNorm(+LIEM)
 kernels.  The (b t)(h w) c <-> (b h w) t c rearranges of the reference
 (ref :307,:314,:1045-1086) do not exist: both are stride views of the same

@@ -10,7 +10,7 @@ class _Cfg(dict):
         self.__dict__ = self
 
 
-cfg = _Cfg(__name__="Config: STAR sm_100a")
+cfg = _Cfg(__name__="Config: STAR sm_90a")
 cfg.model_path = None
 cfg.negative_prompt = ("painting, oil painting, illustration, drawing, art, sketch, oil painting, cartoon, "
                        "CG Style, 3D render, unreal engine, blurring, dirty, messy, worst quality, low quality, "

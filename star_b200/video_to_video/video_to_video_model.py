@@ -4,11 +4,11 @@ Mirrors ``VideoToVideo_sr`` of the reference's video_to_video/video_to_video_mod
 (:20-139: constructor, ``test``; :141-161 VAE helpers; :164-210 ``pad_to_fit`` /
 ``make_chunks`` / ``sliding_windows_1d``).  What differs:
 
-* the denoiser is star_b200's ``ControlledV2VUNet`` (sm_100a kernels), not autocast PyTorch;
+* the denoiser is star_b200's ``ControlledV2VUNet`` (sm_90a kernels), not autocast PyTorch;
 * the diffusion block of ``test`` (ref :98-123) is factored into ``denoise_latents`` so that
   the latent-in / latent-out hot path can be driven (and benchmarked) without the VAE;
 * the temporal VAE is star_b200's own ``AutoencoderKLTemporalDecoder`` (modules/temporal_vae.py, same
-  checkpoint layout as diffusers', sm_100a kernels), loaded from ``opt.vae_path`` (no hub download);
+  checkpoint layout as diffusers', sm_90a kernels), loaded from ``opt.vae_path`` (no hub download);
 * the text encoder (open_clip) is an un-vendored third-party package: it is imported lazily, and
   ready-made objects can be injected (``text_encoder=``, ``vae=``, ``generator=``), which is how the
   tests and the benchmark run on boxes without those packages or checkpoints;
@@ -104,7 +104,7 @@ class VideoToVideo_sr():
 
         if vae is None:
             # ref :57-63 downloads stabilityai/stable-video-diffusion-img2vid (subfolder vae, variant fp16) through
-            # diffusers; here the same checkpoint is read from a local snapshot into the sm_100a temporal VAE.
+            # diffusers; here the same checkpoint is read from a local snapshot into the sm_90a temporal VAE.
             from .modules.temporal_vae import AutoencoderKLTemporalDecoder
             vae_path = _find_vae_dir(opt)
             if vae_path is None:

@@ -14,7 +14,7 @@ def pytest_configure(config):
     import torch
     torch.backends.cudnn.allow_tf32 = False
     torch.backends.cuda.matmul.allow_tf32 = False
-    config.addinivalue_line("markers", "gpu: needs a CUDA (sm_100) device")
+    config.addinivalue_line("markers", "gpu: needs a CUDA (sm_90) device")
     config.addinivalue_line("markers", "reference: needs the reference tree at /root/reference (build container only)")
 
 

@@ -1,9 +1,13 @@
 """CogVideoX-5B DiT layer (STAR's patched block).  PARITY UNPINNED: the oracle (oracle/cogvideox_ref.py) restates
 STAR's layer_forward on top of sat's default leaf modules, which are not in the reference tree."""
+import os
+
 import pytest
 import torch
 
 from tests.util import rel_l2
+
+GOLD = os.path.join(os.path.dirname(__file__), "golden", "reference_checks.pt")
 
 
 def _setup(cfg_kw, seed=3):
@@ -60,43 +64,56 @@ def test_dit_layer_gpu(cfg_kw):
 
 # ------------------------------------------------------------------------------------------------------------------
 # Whole DiffusionTransformer (patch embed, text proj, time embed, N layers with LoRA, final LayerNorm, final layer,
-# unpatchify) against the REFERENCE'S OWN FILES executed behind the sat shim (oracle/cogvideox_sat.py).  Needs the
-# reference tree (/root/reference or the staged oracle/_ref): marker `reference`.
+# unpatchify) against the REFERENCE'S OWN FILES executed behind the sat shim (oracle/cogvideox_sat.py): the CPU tests read
+# the reference outputs from tests/golden/reference_checks.pt (oracle/make_golden_reference.py); the full-width GPU test
+# needs the reference tree (oracle/_ref): marker `reference`.
 SMALL_DIT = dict(num_layers=2, hidden_size=128, num_attention_heads=2, num_frames=9, latent_height=8, latent_width=12,
                  text_length=6, text_hidden_size=32, lora_r=8, time_embed_dim=64)
 
 
-def _dit_pair(kw, dtype, device, seed=4):
-    """(reference net with a synthetic non-zero state dict, star_b200 net with the same weights, inputs)"""
-    from oracle import cogvideox_sat as S
-    from star_b200.cogvideox import DiffusionTransformer
+def dit_state_dict(rec, seed=4):
+    """synthetic non-zero weights for the state-dict manifest rec["manifest"] (the reference's rotary tables rec["freqs"] as is)"""
     from star_b200.utils.synth import synth_tensor
-    ref = S.build_reference_dit(**kw)
     sd = {}
-    for k, v in ref.state_dict().items():
-        if "freqs_" in k:
-            sd[k] = v
+    for k, shape in rec["manifest"].items():
+        if k in rec["freqs"]:
+            sd[k] = rec["freqs"][k]
             continue
-        t = synth_tensor(k, v.shape, seed)
+        t = synth_tensor(k, torch.Size(shape), seed)
         if k.endswith("temp_local.conv1.weight") or k.endswith("spa_local.conv1.weight"):
             t = t * 0.5
         if ".matrix_B." in k:                              # LoRA B is zero-initialised by sat: make the merge matter
             t = t * 8.0
         sd[k] = t
-    ref.load_state_dict(sd)
-    ref = ref.to(device)
-    net = DiffusionTransformer(**kw, dtype=dtype)
-    net.load_state_dict(sd)
-    net = net.to(device)
+    return sd
+
+
+def dit_inputs(kw, device):
     g = torch.Generator().manual_seed(1)
     frames = (kw["num_frames"] - 1) // 4 + 1
     x = torch.randn(2, frames, 32, kw["latent_height"], kw["latent_width"], generator=g).to(device)
     ctx = torch.randn(2, kw["text_length"], kw["text_hidden_size"], generator=g).to(device)
     t = torch.tensor([731, 12]).to(device)
-    return ref, net, x, t, ctx
+    return x, t, ctx
 
 
-@pytest.mark.reference
+def _dit_net(kw, rec, dtype, device):
+    from star_b200.cogvideox import DiffusionTransformer
+    net = DiffusionTransformer(**kw, dtype=dtype)
+    net.load_state_dict(dit_state_dict(rec))
+    return net.to(device)
+
+
+def _dit_pair(kw, dtype, device):
+    """(reference net with a synthetic non-zero state dict, star_b200 net with the same weights, inputs)"""
+    from oracle import cogvideox_sat as S
+    ref = S.build_reference_dit(**kw)
+    rec = {"manifest": {k: tuple(v.shape) for k, v in ref.state_dict().items()},
+           "freqs": {k: v for k, v in ref.state_dict().items() if "freqs_" in k}}
+    ref.load_state_dict(dit_state_dict(rec))
+    return (ref.to(device), _dit_net(kw, rec, dtype, device)) + dit_inputs(kw, device)
+
+
 def test_dit_model_host_graph_vs_reference_files(monkeypatch):
     """CPU: star_b200's host graph (im2col patch embed, LoRA merge, adaLN folding, layer stack, final layer, unpatchify) on the
     emulated kernels against the reference's unmodified DiffusionTransformer (sat shimmed)."""
@@ -105,8 +122,10 @@ def test_dit_model_host_graph_vs_reference_files(monkeypatch):
     for name in dir(KR):
         if not name.startswith("_") and callable(getattr(KR, name)) and hasattr(ops, name):
             monkeypatch.setattr(ops, name, getattr(KR, name))
-    ref, net, x, t, ctx = _dit_pair(SMALL_DIT, torch.float16, "cpu")
-    want = ref(x, timesteps=t, context=ctx)
+    rec = torch.load(GOLD)["dit_small"]
+    net = _dit_net(SMALL_DIT, rec, torch.float16, "cpu")
+    x, t, ctx = dit_inputs(SMALL_DIT, "cpu")
+    want = rec["want"]
     got = net(x, timesteps=t, context=ctx)
     assert got.shape == want.shape == (2, 3, 16, 8, 12)
     err = rel_l2(got, want)
@@ -114,14 +133,13 @@ def test_dit_model_host_graph_vs_reference_files(monkeypatch):
     assert err < 3e-3
 
 
-@pytest.mark.reference
 def test_restated_layer_oracle_is_pinned_to_reference_files():
     """oracle/cogvideox_ref.py (the line-by-line restatement the layer tests use) == the reference's layer_forward"""
     from oracle.cogvideox_ref import DiTCfg, dit_layer_forward
     from star_b200.cogvideox import rope_tables
-    kw = dict(SMALL_DIT, num_layers=1, lora_r=0)
-    ref, _, x, t, ctx = _dit_pair(kw, torch.float16, "cpu")
-    sd = ref.state_dict()
+    gold = torch.load(GOLD)
+    rec = dict(gold["dit_layer"], freqs={k: gold["dit_small"]["freqs"][k] for k in gold["dit_layer"]["freqs"]})
+    sd = dit_state_dict(rec)
     cfg = DiTCfg(hidden=128, heads=2, text_length=6, frames=3, height=4, width=6)
     lsd = {"adaLN_modulation.1.weight": sd["mixins.adaln_layer.adaLN_modulations.0.1.weight"],
            "adaLN_modulation.1.bias": sd["mixins.adaln_layer.adaLN_modulations.0.1.bias"]}
@@ -134,9 +152,7 @@ def test_restated_layer_oracle_is_pinned_to_reference_files():
     g = torch.Generator().manual_seed(2)
     hidden, emb = torch.randn(2, 6 + 72, 128, generator=g), torch.randn(2, 64, generator=g)
     cos, sin = rope_tables(3, 4, 6, 64)
-    ref.transformer.hooks.clear()
-    ref.transformer.hooks.update(ref.hooks)              # what BaseModel.forward does before every call
-    want = ref.hooks["layer_forward"](hidden, torch.ones(1, 1), layer_id=0, emb=emb, text_length=6)
+    want = rec["want"]
     got = dit_layer_forward(lsd, hidden, emb, cfg, cos, sin)
     assert rel_l2(got, want) < 1e-5
 

@@ -21,41 +21,44 @@ class FakeDiT(torch.nn.Module):
         return torch.tanh(0.8 * noisy - 0.3 * lq + 0.1 * noisy.mean(dim=1, keepdim=True)) * (1.0 + 0.2 * c) + 0.05 * t * lq
 
 
-@pytest.mark.reference
 def test_step_plan_matches_reference_tables():
-    from oracle.cogvideox_sampler import build_reference_sampler
+    """against the reference sampler's tables (tests/golden/cogvideox_path.pt, oracle/make_golden_cogvideox.py): alphas_cumprod_sqrt
+    and timesteps of prepare_sampling_loop, the denoiser's quantised sigma and DynamicCFG's scale of every step"""
+    import os
     from star_b200.cogvideox.sampling import StepPlan
-    sampler, denoiser = build_reference_sampler()
-    x = torch.zeros(1, 2, 16, 4, 4)
-    _, s_in, acs, num_sigmas, _, _, timesteps = sampler.prepare_sampling_loop(x, {}, None, None)
+    gold = torch.load(os.path.join(os.path.dirname(__file__), "golden", "cogvideox_path.pt"))
+    acs, timesteps = gold["acs"], gold["timesteps"]
     plan = StepPlan()
-    assert num_sigmas == 51 and torch.equal(plan.alphas_cumprod_sqrt, acs)
-    assert plan.timesteps == [int(t) for t in timesteps]
+    assert len(acs) == 51 and torch.equal(plan.alphas_cumprod_sqrt, acs)
+    assert plan.timesteps == timesteps
     for i, st in enumerate(plan.steps):                                   # quantised sigma of the denoiser, guidance scale
-        q = denoiser.possibly_quantize_sigma(acs[i:i + 1])
-        assert st.c_skip == float(q) and st.timestep == int(timesteps[-(i + 1)])
-        assert st.cfg_scale == sampler.guider.scale_schedule(None, 50 - st.timestep)
+        assert st.c_skip == float(gold["sigma_q"][i]) and st.timestep == timesteps[-(i + 1)]
+        assert st.cfg_scale == gold["cfg"][i]
     assert [st.last for st in plan.steps] == [False] * 49 + [True]
 
 
-@pytest.mark.reference
-@pytest.mark.parametrize("steps", [50, 6])
-def test_sampler_matches_reference(steps):
-    from oracle.cogvideox_sampler import build_reference_sampler, reference_sample
-    from star_b200.cogvideox.sampling import VPSDEDPMPP2MSampler
+def sampler_case():
     g = torch.Generator().manual_seed(0)
     lq = torch.randn(1, 3, 16, 6, 8, generator=g)
     randn = torch.randn(1, 3, 16, 6, 8, generator=g)
     cond = {"crossattn": torch.randn(1, 226, 32, generator=g)}
     uc = {"crossattn": torch.zeros(1, 226, 32)}
-    ref_sampler, ref_den = build_reference_sampler(num_steps=steps)
-    net_r, net_m = FakeDiT(), FakeDiT()
-    torch.manual_seed(123)
-    want = reference_sample(net_r, ref_sampler, ref_den, randn.clone(), dict(cond), dict(uc), lq)
+    return lq, randn, cond, uc
+
+
+@pytest.mark.parametrize("steps", [50, 6])
+def test_sampler_matches_reference(steps):
+    """against the reference sampler's output on the same inputs (tests/golden/reference_checks.pt)"""
+    import os
+    from star_b200.cogvideox.sampling import VPSDEDPMPP2MSampler
+    rec = torch.load(os.path.join(os.path.dirname(__file__), "golden", "reference_checks.pt"))[f"sampler{steps}"]
+    lq, randn, cond, uc = sampler_case()
+    want = rec["want"]
+    net_m = FakeDiT()
     mine = VPSDEDPMPP2MSampler(num_steps=steps, dtype=torch.float32)
     torch.manual_seed(123)
     got = mine(net_m, randn.clone(), cond, uc=uc, lq=torch.cat((lq, lq), 0))
-    assert net_m.calls == net_r.calls and len(net_m.calls) == steps
+    assert net_m.calls == rec["calls"] and len(net_m.calls) == steps
     assert got.shape == want.shape == randn.shape
     assert rel_l2(got, want) < 2e-5
     # random-stream consumption: 1 draw in the first step, 2 in every later one but the last (sampling.py:635,:641)
@@ -95,31 +98,43 @@ def _reference_pipeline(ref_dit, ref_vae, cond, uc, lq, steps, seed, scale_facto
     return torch.clamp((frames + 1.0) / 2.0, 0.0, 1.0), z
 
 
-@pytest.mark.reference
+def pipeline_case(ctx):
+    cond, uc = {"crossattn": ctx[:1]}, {"crossattn": torch.zeros_like(ctx[:1])}
+    lq = torch.rand(1, 9, 3, 64, 96, generator=torch.Generator().manual_seed(9)) * 2 - 1          # LQ clip, already upsampled
+    return cond, uc, lq
+
+
 def test_cogvideox_pipeline_host_graph_on_emulated_kernels(monkeypatch):
     """LQ frames -> frames through 3-D VAE encode + DiT + sampler + 3-D VAE decode (reduced sizes, 4 steps) against the same chain of
-    reference modules"""
+    reference modules (tests/golden/reference_checks.pt: the final latent, and the frames at the seeded sample positions)"""
+    import os
     from oracle import kernel_ref as KR
     from star_b200 import ops
     from star_b200.cogvideox import sample_sr
-    from tests.test_cogvideox import SMALL_DIT
-    from tests.test_cogvideox_vae import SMALL
+    from star_b200.cogvideox.vae3d import ContextParallelDecoder3D, ContextParallelEncoder3D
+    from tests.test_cogvideox import SMALL_DIT, _dit_net, dit_inputs
+    from tests.test_cogvideox_vae import SMALL, decoder_state_dict, encoder_state_dict, sample_positions
     for name in dir(KR):
         if not name.startswith("_") and callable(getattr(KR, name)) and hasattr(ops, name):
             monkeypatch.setattr(ops, name, getattr(KR, name))
-    ref_dit, net, ref_vae, (enc, dec), ctx = _pipeline_pair(SMALL_DIT, SMALL, torch.float16, "cpu")
-    cond, uc = {"crossattn": ctx[:1]}, {"crossattn": torch.zeros_like(ctx[:1])}
-    lq = torch.rand(1, 9, 3, 64, 96, generator=torch.Generator().manual_seed(9)) * 2 - 1          # LQ clip, already upsampled
-    want, z_ref = _reference_pipeline(ref_dit, ref_vae, cond, uc, lq, steps=4, seed=77)
+    gold = torch.load(os.path.join(os.path.dirname(__file__), "golden", "reference_checks.pt"))
+    net = _dit_net(SMALL_DIT, gold["dit_small"], torch.float16, "cpu")
+    _, _, ctx = dit_inputs(SMALL_DIT, "cpu")
+    dec, enc = ContextParallelDecoder3D(**SMALL), ContextParallelEncoder3D(**SMALL)
+    dec.load_state_dict(decoder_state_dict(dec.state_dict()))
+    enc.load_state_dict(encoder_state_dict(enc.state_dict()))
+    dec, enc = dec.to(dtype=torch.float16).eval(), enc.to(dtype=torch.float16).eval()
+    cond, uc, lq = pipeline_case(ctx)
+    want = gold["pipeline"]
     got, z = sample_sr(net, dec, cond, uc, lq=lq, encoder=enc, num_steps=4, seed=77)
-    assert got.shape == want.shape == (1, 9, 3, 64, 96)
-    assert rel_l2(z, z_ref) < 1e-2 and rel_l2(got, want) < 1e-2
+    assert tuple(got.shape) == want["shape"] == (1, 9, 3, 64, 96)
+    assert rel_l2(z, want["z"]) < 1e-2 and rel_l2(got.flatten()[sample_positions(got.numel())], want["frames"]) < 1e-2
 
 
 @pytest.mark.gpu
 @pytest.mark.reference
 def test_cogvideox_pipeline_gpu():
-    """the same chain on the B200 kernels: full-width DiT (2 layers), full-width 3-D VAE decoder, 6 sampler steps, fp16"""
+    """the same chain on the GPU kernels: full-width DiT (2 layers), full-width 3-D VAE decoder, 6 sampler steps, fp16"""
     from oracle.cogvideox_vae import vae_reference_available
     from oracle.cogvideox_sampler import sampler_reference_available
     from star_b200.cogvideox import sample_sr

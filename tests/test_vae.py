@@ -156,7 +156,7 @@ def test_encode_gpu(case):
 @pytest.mark.gpu
 def test_pixel_pipeline_gpu():
     """VideoToVideo_sr.test() end to end on the GPU (row a1) AGAINST THE ORACLE: the same entry is run twice, once on
-    the product members (sm_100a UNet + temporal VAE, fused bilinear+pad and CFG kernels) and once on oracle members (fp32
+    the product members (sm_90a UNet + temporal VAE, fused bilinear+pad and CFG kernels) and once on oracle members (fp32
     restatements: oracle/unet_ref.py -- pinned to the reference -- and oracle/temporal_vae_ref.py -- unpinned) with the
     same seed, so both consume identical posterior / diffuse / SDE noise.  Bilinear x2 upscale + pad_to_fit (720x1280
     canvas -> latent 90x160), per-frame encode, 4-step 'normal' sampler with CFG 7.5, 3-frame decode windows, crop."""

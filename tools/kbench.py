@@ -10,7 +10,7 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-if "--lib" in sys.argv:                       # A/B variant built by tools/build_variant.py
+if "--lib" in sys.argv:                       # A/B: a variant build of the library
     i = sys.argv.index("--lib")
     import star_b200.lib as _lib
     _lib.LIB_PATH = os.path.abspath(sys.argv[i + 1])

@@ -1,12 +1,12 @@
 #!/usr/bin/env python
-"""The UNMODIFIED reference modules on the B200, beside star_b200, on identical weights and inputs.
+"""The UNMODIFIED reference modules on the GPU, beside star_b200, on identical weights and inputs.
 
 What the north-star's ">= 8x the reference's single-GPU PyTorch frames/sec" and "within 1e-3 relative fp16
 tolerance" are written against (BASELINE.md 3/4, SURVEY 8d, VERDICT r1 items 1-2):
 
   * reference fp16 : ControlledV2VUNet().half() under torch.autocast('cuda', fp16), exactly as
                      video_to_video_model.py:42,98 runs it; xformers.memory_efficient_attention is shimmed to
-                     F.scaled_dot_product_attention (xformers 0.0.21 has no sm_100 build) -- timed.
+                     F.scaled_dot_product_attention (xformers is not installed) -- timed.
   * reference fp32 : the same modules in fp32 with TF32 OFF (cudnn + matmul) and an exact chunked fp32
                      attention in place of the fused kernel -- the oracle both fp16 paths are measured against.
   * star_b200      : this repo's forward through the C ABI -- timed, compared with both.
