@@ -86,7 +86,8 @@ int star_attention_causal(const void* Q, long long ldq, const void* K, long long
                           long long ldo, int batch, int heads, int N, float scale, void* stream);
 
 /* Temporal self-attention over T frames per pixel; QKV [B*T*HW, ld] with q|k|v at column 0|Ci|2Ci
- * (unet_v2v.py:483-489 through :158-195). */
+ * (unet_v2v.py:483-489 through :158-195).  Any T >= 1: T <= 64 runs the mma.sync kernel (tattn2.cuh), T > 64 the
+ * wgmma kernel (tattn_long.cuh; needs heads*64 <= Ci <= ld/3, B*HW*heads < 2^31 and T*HW*ld*2 bytes < 2^40). */
 int star_temporal_attention(const void* QKV, long long ld, void* O, long long ldo, int B, int T, long long HW,
                             int heads, int Ci, float scale, void* stream);
 

@@ -15,6 +15,7 @@
 #include "attn.cuh"
 #include "rowops.cuh"
 #include "tattn2.cuh"
+#include "tattn_long.cuh"
 #include "tapgemm.cuh"
 
 using namespace star;
@@ -218,6 +219,7 @@ static int star_init_on_current(int device) {
     STAR_SMEM_ATTR(temporal_attn2_kernel<32>, TA2_WARPS * 3 * 32 * TA2_PITCH);
     STAR_SMEM_ATTR(temporal_attn2_kernel<48>, TA2_WARPS * 3 * 48 * TA2_PITCH);
     STAR_SMEM_ATTR(temporal_attn2_kernel<64>, TA2_WARPS * 3 * 64 * TA2_PITCH);
+    STAR_SMEM_ATTR(temporal_attn_long_kernel, TattnLongSmem::TOTAL);
     STAR_SMEM_ATTR(softmax_rows_kernel, 200 * 1024);
 #undef STAR_SMEM_ATTR
     g_sms[device] = prop.multiProcessorCount;
@@ -455,14 +457,38 @@ int star_attention_causal(const void* Q, long long ldq, const void* K, long long
     return attention_impl(Q, ldq, K, ldk, V, ldv, O, ldo, batch, heads, N, N, 1, scale, 1, stream);
 }
 
+// T > 64: the wgmma kernel of tattn_long.cuh, one persistent CTA per SM
+static int temporal_attention_long(const void* QKV, long long ld, void* O, long long ldo, int B, int T, long long HW,
+                                   int heads, int Ci, float scale, long long items, cudaStream_t st) {
+    if (B < 1 || HW < 1 || heads < 1) return fail("star_temporal_attention: empty problem");
+    if (heads * TL_D > Ci || 3ll * Ci > ld) return fail("star_temporal_attention: need heads*64 <= Ci and 3*Ci <= ld");
+    if (items > 0x7fffffffll) return fail("star_temporal_attention: B*HW*heads must be below 2^31");
+    if ((unsigned long long)T * HW * ld * 2 >= (1ull << 40))
+        return fail("star_temporal_attention: T*HW*ld*2 bytes must be below 2^40 (tensor-map stride limit)");
+    CUtensorMap tm;
+    unsigned long long dims[4] = {3ull * Ci, (unsigned long long)T, (unsigned long long)HW, (unsigned long long)B};
+    unsigned long long str[4] = {1, (unsigned long long)(HW * ld), (unsigned long long)ld, (unsigned long long)T * HW * ld};
+    unsigned box[4] = {TL_D, TL_BT, 1, 1};
+    if (make_tmap(&tm, QKV, 4, dims, str, box)) return 1;
+    TattnLongParams p;
+    p.T = T; p.heads = heads; p.HW = (int)HW; p.nitems = (int)items; p.Ci = Ci;
+    p.scale_log2 = scale * 1.4426950408889634f;
+    p.out = (__half*)O; p.ldo = ldo;
+    const unsigned grid = (unsigned)std::min<long long>(items, (long long)num_sms());
+    temporal_attn_long_kernel<<<grid, TL_THREADS, TattnLongSmem::TOTAL, st>>>(tm, p);
+    STAR_LAUNCH_CHECK("temporal_attn_long");
+    return 0;
+}
+
 int star_temporal_attention(const void* QKV, long long ld, void* O, long long ldo, int B, int T, long long HW,
                             int heads, int Ci, float scale, void* stream) {
     STAR_CHECK_INIT();
-    if (T > TA2_MAXT || T < 1) return fail("star_temporal_attention: T=%d outside [1, %d]", T, TA2_MAXT);
+    if (T < 1) return fail("star_temporal_attention: T=%d must be >= 1", T);
     if (ld % 8 || ldo % 8 || Ci % 8) return fail("star_temporal_attention: ld/ldo/Ci must be multiples of 8");
     if ((reinterpret_cast<uintptr_t>(QKV) | reinterpret_cast<uintptr_t>(O)) % 16) return fail("star_temporal_attention: pointers must be 16-byte aligned");
     const long long items = (long long)B * HW * heads;
     cudaStream_t st = (cudaStream_t)stream;
+    if (T > TA2_MAXT) return temporal_attention_long(QKV, ld, O, ldo, B, T, HW, heads, Ci, scale, items, st);
     const int tp = (T + 15) / 16 * 16;
     const unsigned grid = (unsigned)std::min<long long>((items + TA2_WARPS - 1) / TA2_WARPS, (long long)num_sms() * 2);
     const size_t smem = (size_t)TA2_WARPS * 3 * tp * TA2_PITCH;

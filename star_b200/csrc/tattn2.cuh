@@ -1,5 +1,7 @@
 // star_b200 / csrc / tattn2.cuh
-// Temporal self-attention over T <= 64 frames per (pixel, head) (unet_v2v.py:483-489), second version.
+// Temporal self-attention over T <= 64 frames per (pixel, head) (unet_v2v.py:483-489), second version.  Chunks of
+// T > 64 frames (max_chunk_len >= 52) run temporal_attn_long_kernel (tattn_long.cuh, wgmma); star_temporal_attention
+// picks the kernel by T.
 // The problem is a 32x32x64 attention per item, 131 760 items per call at level 0: HBM-bound (the q|k|v
 // rows of a pixel are 128-byte segments strided by H*W rows).  v1 did the two small matmuls on the FMA
 // pipes with per-element fp16->fp32 converts and was instruction-bound (988 GB/s).  Here one warp handles

@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """Kernel micro-benchmarks at the shapes of BASELINE config 2 (32 frames, latent 122x216).
 CUDA events, 2 warm-up + N timed launches per shape; prints ms, TFLOP/s or GB/s and the fraction of the
-measured peak (MEASURED_PEAKS.json).  Usage: python tools/kbench.py [attention linear conv ...]"""
+measured peak (MEASURED_PEAKS.json), or of the H100 SXM data sheet (989 TFLOP/s dense fp16, 3.35 TB/s HBM3) where no
+measured peak is present.  Usage: python tools/kbench.py [attention linear conv rowops tattn ...]"""
 import json
 import os
 import sys
@@ -18,11 +19,13 @@ if "--lib" in sys.argv:                       # A/B: a variant build of the libr
     print("# library:", _lib.LIB_PATH)
 from star_b200 import ops as O  # noqa: E402
 
-PEAK = {"tflops": 1717.6, "gbs": 6576.1}
+PEAK = {"tflops": 989.0, "gbs": 3350.0}                          # H100 SXM data sheet (700 W)
+PEAK_SRC = ("data sheet", "data sheet")
 p = os.path.join(ROOT, "MEASURED_PEAKS.json")
 if os.path.isfile(p):
     d = json.load(open(p))
     PEAK = {"tflops": d["bf16_tflops"], "gbs": d["hbm_gbs"]}      # kernels timed alone: burst figures
+    PEAK_SRC = ("measured burst", "measured copy")
 
 
 def rnd(*shape, scale=1.0):
@@ -46,10 +49,10 @@ def report(name, ms, flops=None, bytes_=None):
     s = f"{name:58s} {ms:9.3f} ms"
     if flops:
         tf = flops / ms / 1e9
-        s += f"  {tf:8.1f} TFLOP/s ({100 * tf / PEAK['tflops']:5.1f}% of measured burst)"
+        s += f"  {tf:8.1f} TFLOP/s ({100 * tf / PEAK['tflops']:5.1f}% of {PEAK_SRC[0]})"
     if bytes_:
         gb = bytes_ / ms / 1e6
-        s += f"  {gb:8.1f} GB/s ({100 * gb / PEAK['gbs']:5.1f}% of measured copy)"
+        s += f"  {gb:8.1f} GB/s ({100 * gb / PEAK['gbs']:5.1f}% of {PEAK_SRC[1]})"
     print(s, flush=True)
 
 
@@ -135,6 +138,32 @@ def bench_rowops():
     report("concat_add 320|320", timeit(lambda: O.concat_add(a, bb, bb)), bytes_=5.0 * R * 320 * 2)
 
 
+def bench_tattn():
+    """Temporal attention at level 0 of a 960p latent (26 352 pixels, 5 heads, Ci 320) over T frames: T <= 64 runs
+    temporal_attn2_kernel (tattn2.cuh), T > 64 temporal_attn_long_kernel (tattn_long.cuh).  Bytes = QKV read + O write,
+    FLOP = 4 T^2 64 per (pixel, head); the floor is the larger of bytes / peak bandwidth and FLOP / peak rate."""
+    HW, heads, C = 26352, 5, 320
+    for T in (32, 64, 65, 78, 128):
+        qkv = rnd(T * HW, 3 * C)
+        flops, bytes_ = 4.0 * T * T * 64 * HW * heads, 4.0 * T * HW * C * 2
+        ms = timeit(lambda: O.temporal_attention(qkv, 1, T, HW, heads, C), 20)
+        t_hbm, t_mma = bytes_ / (PEAK["gbs"] * 1e6), flops / (PEAK["tflops"] * 1e9)
+        report(f"temporal attention L0 T={T} HW={HW} heads={heads}", ms, flops=flops, bytes_=bytes_)
+        print(f"{'':58s} floor {max(t_hbm, t_mma):.3f} ms ({'HBM' if t_hbm >= t_mma else 'MMA'}-bound), "
+              f"achieved {100 * max(t_hbm, t_mma) / ms:5.1f}% of it", flush=True)
+        del qkv
+
+
+def card():
+    import subprocess
+    try:
+        o = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                           capture_output=True, text=True, timeout=10).stdout.strip()
+        print(f"# card: {o}", flush=True)
+    except Exception as e:
+        print("# nvidia-smi failed", e)
+
+
 def clocks():
     import subprocess
     try:
@@ -147,7 +176,8 @@ def clocks():
 
 if __name__ == "__main__":
     which = sys.argv[1:] or ["attention", "linear", "conv", "rowops"]
-    print(f"# peaks used: {PEAK}")
+    card()
+    print(f"# peaks used: {PEAK} ({PEAK_SRC[0]} / {PEAK_SRC[1]})")
     for w in which:
         globals()["bench_" + w]()
         clocks()
