@@ -180,6 +180,16 @@ long long star_cfg_x0_workspace_bytes(int samples);
 int star_cfg_x0(const void* y_out, const void* u_out, const void* xt_f32, void* x0_f32, void* guided_out,
                 float guide_scale, float guide_rescale, const void* alpha_f32, const void* sigma_f32, int samples,
                 long long per_sample, void* workspace, void* stream);
+/* star_cfg_x0 for one (temporal chunk, spatial tile) model call of tiled sampling, accumulated into the clip's x0:
+ *   acc[s, c, f0 + f, r0 + i, c0 + j] += wy[i] * wx[j] * x0[s, c, f, i, j]      for lo <= f < hi
+ * y_out / u_out fp16 [samples, C, Ft, th, tw] contiguous (the tile's outputs; the std-ratio statistics span all Ft frames);
+ * xt_f32 / acc_f32 fp32 [samples, C, F, H, W] contiguous (the clip, read / updated in place at the window); wy [th], wx [tw]
+ * fp32 blend weights on the device.  A unit weight into a zeroed acc gives star_cfg_x0's x0 bit for bit.  Each tile sample
+ * must have fewer than 2^31 elements.  workspace: star_cfg_x0_workspace_bytes(samples). */
+int star_cfg_x0_blend(const void* y_out, const void* u_out, const void* xt_f32, void* acc_f32, float guide_scale,
+                      float guide_rescale, const void* alpha_f32, const void* sigma_f32, const void* wy_f32, const void* wx_f32,
+                      int samples, int C, int Ft, int th, int tw, int F, int H, int W, int f0, int lo, int hi, int r0, int c0,
+                      void* workspace, void* stream);
 /* sinusoidal timestep embedding (unet_v2v.py:96-108); t = int64 [B]; out fp16 [B, dim] */
 int star_sinusoidal(const void* t_i64, void* out, int B, int dim, void* stream);
 int star_silu(const void* x, void* out, long long n, void* stream);

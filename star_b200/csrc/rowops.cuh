@@ -1129,4 +1129,48 @@ cfg_x0_kernel(const __half* __restrict__ y, const __half* __restrict__ u, const 
     }
 }
 
+// Spatially tiled sampling: the same guided x0 for one (chunk, tile) model call, accumulated into the clip-level x0 with the
+// tile's separable blend weights: acc[b, c, f0 + f, r0 + i, c0 + j] += wy[i] * wx[j] * x0 for the kept frames lo <= f < hi.
+// y / u: [samples][C][Ft][th][tw] (the tile), xt / acc: [samples][C][F][H][W] (the clip), read and written in place.
+// Element order and rounding of x0 are cfg_x0_kernel's, so a unit weight into a zeroed acc reproduces it bit for bit.
+struct CfgBlendGeom {
+    int C, Ft, th, tw, lo, hi;                  // tile extents and kept frame range (tile-local)
+    long long F, H, W, f0, r0, c0;              // clip extents and the tile's window offset
+};
+
+__global__ void __launch_bounds__(256)
+cfg_x0_blend_kernel(const __half* __restrict__ y, const __half* __restrict__ u, const float* __restrict__ xt,
+                    float* __restrict__ acc, float g, float r, int has_rescale, const float* __restrict__ alpha,
+                    const float* __restrict__ sigma, const float* __restrict__ wy, const float* __restrict__ wx,
+                    CfgBlendGeom q, const double* __restrict__ stats) {
+    const int sample = blockIdx.y;
+    const unsigned per_sample = (unsigned)q.C * q.Ft * q.th * q.tw;
+    float scale = 1.f;
+    if (has_rescale) {
+        const double n = (double)per_sample;
+        const double vy = (stats[sample * 4 + 1] - stats[sample * 4 + 0] * stats[sample * 4 + 0] / n) / (n - 1.0);
+        const double vo = (stats[sample * 4 + 3] - stats[sample * 4 + 2] * stats[sample * 4 + 2] / n) / (n - 1.0);
+        const float sdy = __half2float(__float2half_rn((float)sqrt(vy > 0.0 ? vy : 0.0)));
+        const float sdo = __half2float(__float2half_rn((float)sqrt(vo > 0.0 ? vo : 0.0)));
+        const float ratio = __half2float(__float2half_rn(__fdiv_rn(sdy, __half2float(__float2half_rn(sdo + 1e-12f)))));
+        const float a = __half2float(__float2half_rn(r * ratio));
+        scale = __half2float(__float2half_rn(a + (1.f - r)));
+    }
+    const float al = alpha[sample], sg = sigma[sample];
+    const unsigned nf = (unsigned)(q.hi - q.lo), plane = (unsigned)q.th * q.tw;
+    const unsigned kept = (unsigned)q.C * nf * plane;
+    const long long tile_base = (long long)sample * per_sample;
+    for (unsigned k = blockIdx.x * blockDim.x + threadIdx.x; k < kept; k += gridDim.x * blockDim.x) {
+        const unsigned j = k % q.tw, ij = k / q.tw;
+        const unsigned i = ij % q.th, cf = ij / q.th;
+        const unsigned f = q.lo + cf % nf, c = cf / nf;
+        const long long src = tile_base + ((long long)(c * q.Ft + f) * plane + i * q.tw + j);
+        const long long dst = (((long long)sample * q.C + c) * q.F + q.f0 + f) * q.H * q.W + (q.r0 + i) * q.W + q.c0 + j;
+        float o = cfg_combine_h(y[src], u[src], g);
+        if (has_rescale) o = __half2float(__float2half_rn(o * scale));
+        const float x0 = __fsub_rn(__fmul_rn(al, xt[dst]), __fmul_rn(sg, o));
+        acc[dst] = __fmaf_rn(__fmul_rn(wy[i], wx[j]), x0, acc[dst]);
+    }
+}
+
 }  // namespace star

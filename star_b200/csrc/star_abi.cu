@@ -787,6 +787,47 @@ int star_cfg_x0(const void* y_out, const void* u_out, const void* xt_f32, void* 
     return 0;
 }
 
+int star_cfg_x0_blend(const void* y_out, const void* u_out, const void* xt_f32, void* acc_f32, float guide_scale,
+                      float guide_rescale, const void* alpha_f32, const void* sigma_f32, const void* wy_f32, const void* wx_f32,
+                      int samples, int C, int Ft, int th, int tw, int F, int H, int W, int f0, int lo, int hi, int r0, int c0,
+                      void* workspace, void* stream) {
+    if (!y_out || !u_out || !xt_f32 || !acc_f32 || !alpha_f32 || !sigma_f32 || !wy_f32 || !wx_f32)
+        return fail("star_cfg_x0_blend: null pointer");
+    if (samples <= 0 || samples > 65535) return fail("star_cfg_x0_blend: samples=%d outside [1, 65535]", samples);
+    if (C < 1 || Ft < 1 || th < 1 || tw < 1) return fail("star_cfg_x0_blend: empty tile %dx%dx%dx%d", C, Ft, th, tw);
+    if (f0 < 0 || r0 < 0 || c0 < 0 || (long long)f0 + Ft > F || (long long)r0 + th > H || (long long)c0 + tw > W)
+        return fail("star_cfg_x0_blend: window frames [%d, %lld) rows [%d, %lld) cols [%d, %lld) outside the clip %dx%dx%d",
+                    f0, (long long)f0 + Ft, r0, (long long)r0 + th, c0, (long long)c0 + tw, F, H, W);
+    if (lo < 0 || hi > Ft || lo >= hi) return fail("star_cfg_x0_blend: kept frames [%d, %d) outside the tile's %d", lo, hi, Ft);
+    // tile offsets are 32-bit in the kernel; clip offsets 64-bit
+    const long long per_sample = (long long)C * Ft * th * tw;
+    if (per_sample <= 1 || per_sample >= (1ll << 31)) return fail("star_cfg_x0_blend: %lld elements per tile sample outside [2, 2^31)", per_sample);
+    const double clip = (double)samples * C * F * H * W;
+    if (clip >= 9.0e18) return fail("star_cfg_x0_blend: clip of %.3g elements exceeds 64-bit indexing", clip);
+    if (((uintptr_t)y_out | (uintptr_t)u_out) % 2 || ((uintptr_t)xt_f32 | (uintptr_t)acc_f32 | (uintptr_t)alpha_f32 |
+                                                      (uintptr_t)sigma_f32 | (uintptr_t)wy_f32 | (uintptr_t)wx_f32) % 4)
+        return fail("star_cfg_x0_blend: misaligned pointer");
+    cudaStream_t st = (cudaStream_t)stream;
+    const int has_rescale = guide_rescale >= 0.f;
+    double* stats = (double*)workspace;
+    if (has_rescale) {
+        if (!workspace) return fail("star_cfg_x0_blend: the std-ratio rescale needs a workspace");
+        const unsigned gs = (unsigned)std::min<long long>((per_sample + 255) / 256, (long long)num_sms() * 8);
+        STAR_CUDA(cudaMemsetAsync(stats, 0, (size_t)samples * 4 * 8, st));
+        cfg_stats_kernel<<<dim3(gs, samples), 256, 0, st>>>((const __half*)y_out, (const __half*)u_out, guide_scale, per_sample, stats);
+        STAR_LAUNCH_CHECK("cfg_stats");
+    }
+    const long long kept = (long long)C * (hi - lo) * th * tw;
+    const unsigned gx = (unsigned)std::min<long long>((kept + 255) / 256, (long long)num_sms() * 8);
+    CfgBlendGeom q{C, Ft, th, tw, lo, hi, F, H, W, f0, r0, c0};
+    cfg_x0_blend_kernel<<<dim3(gx, samples), 256, 0, st>>>((const __half*)y_out, (const __half*)u_out, (const float*)xt_f32,
+                                                           (float*)acc_f32, guide_scale, guide_rescale, has_rescale,
+                                                           (const float*)alpha_f32, (const float*)sigma_f32, (const float*)wy_f32,
+                                                           (const float*)wx_f32, q, stats);
+    STAR_LAUNCH_CHECK("cfg_x0_blend");
+    return 0;
+}
+
 int star_sinusoidal(const void* t_i64, void* out, int B, int dim, void* stream) {
     const int n = B * (dim / 2);
     sinusoidal_kernel<<<(n + 127) / 128, 128, 0, (cudaStream_t)stream>>>((const long long*)t_i64, (__half*)out, B, dim);

@@ -54,6 +54,7 @@ SIGNATURES = {
     "star_adain_color_fix": (_i, [_p, _p, _p, _p, _i, _i, _ll, _ll, _p, _p]),
     "star_cfg_x0_workspace_bytes": (_ll, [_i]),
     "star_cfg_x0": (_i, [_p, _p, _p, _p, _p, _f, _f, _p, _p, _i, _ll, _p, _p]),
+    "star_cfg_x0_blend": (_i, [_p, _p, _p, _p, _f, _f, _p, _p, _p, _p] + [_i] * 13 + [_p, _p]),
     "star_sinusoidal": (_i, [_p, _p, _i, _i, _p]),
     "star_silu": (_i, [_p, _p, _ll, _p]),
 }

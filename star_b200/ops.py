@@ -5,6 +5,8 @@ only; every op below is one call into libstar_sm100.so.  All activations are
 fp16 CUDA tensors in the channels-last token layout X[rows, C] with rows
 ordered (b, t, h, w).
 """
+from typing import NamedTuple
+
 import torch
 
 from . import lib as _L
@@ -493,11 +495,32 @@ def adain_color_fix(video, source, uint8=False):
     return out
 
 
+class TileBlend(NamedTuple):
+    """Where ``cfg_x0(..., blend=)`` accumulates one (chunk, tile) x0 in tiled sampling: the clip-level fp32 accumulator
+    (B, C, F, H, W), the tile's frame / row / column offset in the clip (f0, r0, c0), the kept tile-local frames [lo, hi)
+    and the tile's fp32 row / column blend weights wy (th,), wx (tw,) on the device."""
+    acc: torch.Tensor
+    f0: int
+    lo: int
+    hi: int
+    r0: int
+    c0: int
+    wy: torch.Tensor
+    wx: torch.Tensor
+
+
 @_traced
-def cfg_x0(y_out, u_out, xt, alphas, sigmas, guide_scale, guide_rescale=None, return_guided=False):
-    """x0 = alphas * xt - sigmas * rescale(u + g (y - u)); y_out / u_out fp16 (B, ...), xt fp32, alphas / sigmas fp32 (B, 1, ...)"""
+def cfg_x0(y_out, u_out, xt, alphas, sigmas, guide_scale, guide_rescale=None, return_guided=False, blend=None):
+    """x0 = alphas * xt - sigmas * rescale(u + g (y - u)); y_out / u_out fp16 (B, ...), xt fp32, alphas / sigmas fp32 (B, 1, ...)
+
+    With ``blend`` (a TileBlend), y_out / u_out are the outputs of one tile (B, C, Ft, th, tw), xt is the CLIP-level latent
+    (B, C, F, H, W) fp32 contiguous, read in place at the tile's window, and x0 is not returned but accumulated:
+    blend.acc[:, :, f0 + lo:f0 + hi, r0:r0 + th, c0:c0 + tw] += wy[:, None] * wx[None, :] * x0[:, :, lo:hi]; returns blend.acc.
+    The rescale statistics span the whole tile output."""
     _dev(y_out)
     _h(y_out, "y_out"); _h(u_out, "u_out")
+    if blend is not None:
+        return _cfg_x0_blend(y_out, u_out, xt, alphas, sigmas, guide_scale, guide_rescale, return_guided, blend)
     assert y_out.is_contiguous() and u_out.is_contiguous() and y_out.shape == u_out.shape == xt.shape
     B = y_out.shape[0]
     per = y_out.numel() // B
@@ -512,6 +535,35 @@ def cfg_x0(y_out, u_out, xt, alphas, sigmas, guide_scale, guide_rescale=None, re
                            -1.0 if guide_rescale is None else float(guide_rescale), _p(al), _p(sg), B, per, _p(ws), _st()),
              "star_cfg_x0")
     return (x0, guided) if return_guided else x0
+
+
+def _cfg_x0_blend(y_out, u_out, xt, alphas, sigmas, guide_scale, guide_rescale, return_guided, blend):
+    if return_guided:
+        raise ValueError("cfg_x0: return_guided is not available with blend=")
+    acc = blend.acc
+    if y_out.dim() != 5 or y_out.shape != u_out.shape or not (y_out.is_contiguous() and u_out.is_contiguous()):
+        raise ValueError(f"cfg_x0(blend=): y_out / u_out must be contiguous (B, C, Ft, th, tw), got {tuple(y_out.shape)} "
+                         f"and {tuple(u_out.shape)}")
+    for name, t in (("xt", xt), ("blend.acc", acc), ("blend.wy", blend.wy), ("blend.wx", blend.wx)):
+        if t.dtype != torch.float32 or not t.is_contiguous() or t.device != y_out.device:
+            raise ValueError(f"cfg_x0(blend=): {name} must be a contiguous fp32 tensor on {y_out.device}")
+    B, C, Ft, th, tw = y_out.shape
+    if xt.dim() != 5 or acc.shape != xt.shape or xt.shape[:2] != (B, C):
+        raise ValueError(f"cfg_x0(blend=): xt {tuple(xt.shape)} and acc {tuple(acc.shape)} must be the same (B, C, F, H, W) clip "
+                         f"as the tile's (B, C) = ({B}, {C})")
+    if blend.wy.shape != (th,) or blend.wx.shape != (tw,):
+        raise ValueError(f"cfg_x0(blend=): weights {tuple(blend.wy.shape)} / {tuple(blend.wx.shape)} do not match the tile {th}x{tw}")
+    _, _, F, H, W = xt.shape
+    al = alphas.reshape(B).float().contiguous()
+    sg = sigmas.reshape(B).float().contiguous()
+    L = _lib()
+    ws = torch.empty(L.star_cfg_x0_workspace_bytes(B), dtype=torch.uint8, device=y_out.device)
+    _L.check(L.star_cfg_x0_blend(_p(y_out), _p(u_out), _p(xt), _p(acc), float(guide_scale),
+                                 -1.0 if guide_rescale is None else float(guide_rescale), _p(al), _p(sg), _p(blend.wy),
+                                 _p(blend.wx), B, C, Ft, th, tw, F, H, W, int(blend.f0), int(blend.lo), int(blend.hi),
+                                 int(blend.r0), int(blend.c0), _p(ws), _st()),
+             "star_cfg_x0_blend")
+    return acc
 
 
 FLAG_GELU_TANH = 8

@@ -79,29 +79,7 @@ class GaussianDiffusion(object):
         var = betas * (sigmas_s / sigmas) ** 2
         log_var = torch.log(var).clamp_(-20, 20)
 
-        if guide_scale is None:
-            assert isinstance(model_kwargs, dict)
-            out = model(xt, t=t, **model_kwargs)
-        else:
-            assert isinstance(model_kwargs, list)
-            pair = getattr(model, "forward_cfg_pair", None)
-            if guide_scale != 1.0 and pair is not None and set(model_kwargs[0]) == set(model_kwargs[1]) == {"y"}:
-                # the two branches differ only in the text embedding: the model evaluates their common, text-independent
-                # prefix once (bit-identical to two calls, tests/test_unet_gpu.py::test_cfg_pair_equals_two_forwards)
-                extra = {}
-                for kw in model_kwargs[2:]:
-                    extra.update(kw)
-                if len(model_kwargs) <= 3:
-                    extra["variant_info"] = variant_info
-                out = pair(xt, t, (model_kwargs[0]["y"], model_kwargs[1]["y"]), **extra)
-            else:
-                y_out = self._branch_out(xt, t, model, model_kwargs, 0, variant_info)
-                if guide_scale == 1.0:
-                    out = y_out
-                else:
-                    u_out = self._branch_out(xt, t, model, model_kwargs, 1, variant_info)
-                    out = (y_out, u_out)
-
+        out = self._model_out(xt, t, model, model_kwargs, guide_scale, variant_info)
         if isinstance(out, tuple):
             x0 = self._guided_x0(out[0], out[1], xt, alphas, sigmas, guide_scale, guide_rescale, clamp, percentile)
         else:
@@ -109,6 +87,28 @@ class GaussianDiffusion(object):
         eps = (xt - alphas * x0) / sigmas
         mu = coef1 * x0 + coef2 * xt
         return mu, var, log_var, x0, eps
+
+    def _model_out(self, xt, t, model, model_kwargs, guide_scale, variant_info):
+        """The model call(s) of one denoise evaluation: the output, or the (conditional, unconditional) pair under CFG."""
+        if guide_scale is None:
+            assert isinstance(model_kwargs, dict)
+            return model(xt, t=t, **model_kwargs)
+        assert isinstance(model_kwargs, list)
+        pair = getattr(model, "forward_cfg_pair", None)
+        if guide_scale != 1.0 and pair is not None and set(model_kwargs[0]) == set(model_kwargs[1]) == {"y"}:
+            # the two branches differ only in the text embedding: the model evaluates their common, text-independent
+            # prefix once (bit-identical to two calls, tests/test_unet_gpu.py::test_cfg_pair_equals_two_forwards)
+            extra = {}
+            for kw in model_kwargs[2:]:
+                extra.update(kw)
+            if len(model_kwargs) <= 3:
+                extra["variant_info"] = variant_info
+            return pair(xt, t, (model_kwargs[0]["y"], model_kwargs[1]["y"]), **extra)
+        y_out = self._branch_out(xt, t, model, model_kwargs, 0, variant_info)
+        if guide_scale == 1.0:
+            return y_out
+        u_out = self._branch_out(xt, t, model, model_kwargs, 1, variant_info)
+        return (y_out, u_out)
 
     @staticmethod
     def _branch_out(xt, t, model, model_kwargs, branch, variant_info):
@@ -156,7 +156,10 @@ class GaussianDiffusion(object):
                   guide_rescale=None, clamp=None, percentile=None, solver='euler_a',
                   solver_mode='fast', steps=20, t_max=None, t_min=None, discretization=None,
                   discard_penultimate_step=None, return_intermediate=None, show_progress=False,
-                  seed=-1, chunk_inds=None, variant_info=None, chunk_parallel="auto", **kwargs):
+                  seed=-1, chunk_inds=None, variant_info=None, chunk_parallel="auto", tile_inds=None, **kwargs):
+        """``tile_inds`` (the output of video_to_video_model.make_tiles) turns on spatially tiled sampling: every solver-step
+        evaluation runs the model on each (chunk, tile) window and blends the windows' x0 into the clip's x0 with the tiles'
+        weights (see _eval_x0_tiled).  Without it, every path below runs on whole frames."""
         assert isinstance(steps, (int, torch.LongTensor))
         assert t_max is None or (0 < t_max <= self.num_timesteps - 1)
         assert t_min is None or (0 <= t_min < self.num_timesteps - 1)
@@ -176,6 +179,9 @@ class GaussianDiffusion(object):
         # SURVEY App. B); a one-window list is the un-chunked case.
         if chunk_inds is not None and len(chunk_inds) < 2:
             chunk_inds = None
+        if tile_inds is not None and dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
+            raise NotImplementedError("sample_sr: tiled sampling runs in a single process; spatial tiles are not sharded "
+                                      "across ranks")
 
         intermediates = []
         world, rank = 1, 0
@@ -259,7 +265,19 @@ class GaussianDiffusion(object):
         if discard_penultimate_step:
             sigmas = torch.cat([sigmas[:-2], sigmas[-1:]])
 
-        if chunk_inds is not None and world > 1 and mode == "literal":
+        if tile_inds is not None:
+            windows = self._tile_windows(noise, chunk_inds, keep, tile_inds, model_kwargs, guide_scale, clamp, percentile)
+
+            def eval_x0_tiled(xt, sigma, variant_info=None):
+                t = self._sigma_to_t(sigma).repeat(len(xt)).round().long()
+                x0 = self._eval_x0_tiled(xt, t, windows, model, model_kwargs, guide_scale, guide_rescale, variant_info)
+                if return_intermediate == 'xt':
+                    intermediates.append(xt)
+                elif return_intermediate == 'x0':
+                    intermediates.append(x0)
+                return x0
+            x0 = solver_fn(noise, eval_x0_tiled, sigmas, variant_info=variant_info, show_progress=show_progress, **kwargs)
+        elif chunk_inds is not None and world > 1 and mode == "literal":
             x0 = self._sample_literal(noise, solver_fn, sigmas, chunk_inds, keep, model, model_kwargs,
                                       guide_scale, guide_rescale, clamp, percentile, variant_info,
                                       world, rank, show_progress, kwargs)
@@ -267,6 +285,51 @@ class GaussianDiffusion(object):
             fn = eval_x0_chunked if chunk_inds is not None else eval_x0
             x0 = solver_fn(noise, fn, sigmas, variant_info=variant_info, show_progress=show_progress, **kwargs)
         return (x0, intermediates) if return_intermediate is not None else x0
+
+    # -- spatially tiled sampling ------------------------------------------------
+    @staticmethod
+    def _tile_windows(noise, chunk_inds, keep, tile_inds, model_kwargs, guide_scale, clamp, percentile):
+        """The (chunk, tile) windows of one evaluation: [(s, e, lo, hi, r0, r1, c0, c1, wy, wx)], frames [s, e) of which the
+        chunk keeps [lo, hi) (chunk-local), rows [r0, r1), cols [c0, c1), and the tile's weights uploaded once per call."""
+        if guide_scale is None or not isinstance(model_kwargs, list) or len(model_kwargs) < 3 \
+                or 'hint' not in model_kwargs[2]:
+            raise ValueError("sample_sr(tile_inds=...): tiled sampling needs classifier-free guidance (guide_scale) and "
+                             "model_kwargs [{'y': ...}, {'y': ...}, {'hint': ...}]")
+        if clamp is not None or percentile is not None:
+            raise NotImplementedError("sample_sr(tile_inds=...): clamp / percentile are not supported")
+        rows, cols, row_w, col_w = tile_inds
+        f = noise.shape[2]
+        chunks = chunk_inds if chunk_inds is not None else [(0, f)]
+        kept = keep if keep is not None else [(0, f)]
+        row_w = [w.to(noise.device, torch.float32).contiguous() for w in row_w]
+        col_w = [w.to(noise.device, torch.float32).contiguous() for w in col_w]
+        return [(s, e, lo, hi, r0, r1, c0, c1, wy, wx)
+                for (s, e), (lo, hi) in zip(chunks, kept)
+                for (r0, r1), wy in zip(rows, row_w)
+                for (c0, c1), wx in zip(cols, col_w)]
+
+    def _eval_x0_tiled(self, xt, t, windows, model, model_kwargs, guide_scale, guide_rescale, variant_info):
+        """x0 of the clip = sum over (chunk, tile) windows of the tile's blend weight times its x0, restricted to the frames
+        the chunk keeps (stitch_slices).  Each window runs the model on the cropped latent and LR latent, with the branch
+        logic of ``denoise``; one star_cfg_x0_blend launch pair per window forms the guided x0 (CFG, std-ratio rescale over
+        the window, v -> x0) and adds it into the clip's x0 in place.  Needs fp16 CUDA model outputs (the .half() UNet)."""
+        from ... import ops
+        xt = xt.float().contiguous()
+        x0 = torch.zeros_like(xt)
+        alphas, sigmas = _gather_coef(self.alphas, t, xt), _gather_coef(self.sigmas, t, xt)
+        hint = model_kwargs[2]['hint']                                    # the clip's LR latent; each window gets its crop
+        rescale = None if guide_scale == 1.0 else guide_rescale        # as denoise: no rescale without a second branch
+        for s, e, lo, hi, r0, r1, c0, c1, wy, wx in windows:
+            kw = [model_kwargs[0], model_kwargs[1],
+                  dict(model_kwargs[2], hint_chunk=hint[:, :, s:e, r0:r1, c0:c1].contiguous())] + list(model_kwargs[3:])
+            out = self._model_out(xt[:, :, s:e, r0:r1, c0:c1].contiguous(), t, model, kw, guide_scale, variant_info)
+            y_out, u_out = out if isinstance(out, tuple) else (out, out)
+            if not (y_out.is_cuda and y_out.dtype == torch.float16 and u_out.dtype == torch.float16):
+                raise TypeError("sample_sr(tile_inds=...): tiled sampling blends on the GPU and needs fp16 CUDA model outputs "
+                                f"(the .half() UNet), got {y_out.dtype} on {y_out.device}")
+            ops.cfg_x0(y_out.contiguous(), u_out.contiguous(), xt, alphas, sigmas, guide_scale, rescale,
+                       blend=ops.TileBlend(x0, s, lo, hi, r0, c0, wy, wx))
+        return x0
 
     # -- chunk-parallel helpers -------------------------------------------------
     @staticmethod

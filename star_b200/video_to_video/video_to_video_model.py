@@ -35,7 +35,7 @@ from .utils.logger import get_logger
 
 logger = get_logger()
 
-__all__ = ["VideoToVideo_sr", "pad_to_fit", "make_chunks", "sliding_windows_1d"]
+__all__ = ["VideoToVideo_sr", "pad_to_fit", "make_chunks", "make_tiles", "sliding_windows_1d"]
 
 
 def _dist_info():
@@ -131,10 +131,15 @@ class VideoToVideo_sr():
     @torch.no_grad()
     def denoise_latents(self, video_data_feature, y, negative_y=None, total_noise_levels=1000, steps=50,
                         solver_mode='fast', guide_scale=7.5, max_chunk_len=32, noise=None, noise_sampler=None,
-                        chunk_parallel="auto"):
+                        chunk_parallel="auto", tile_size=None, tile_overlap=16):
         """video_data_feature: (1,4,F,h,w) VAE latent of the upsampled LR clip (any device; moved to
         self.device), y / negative_y: (1,77,1024).  Returns the denoised latent (1,4,F,h,w) fp32 on
-        self.device.  ``noise`` / ``noise_sampler`` pin the two random inputs (diffuse noise, SDE noise)."""
+        self.device.  ``noise`` / ``noise_sampler`` pin the two random inputs (diffuse noise, SDE noise).
+
+        ``tile_size = (th, tw)`` (latent units, th = 2 and tw = 0 mod 8) denoises overlapping spatial tiles of
+        ``tile_overlap`` latent pixels and blends their x0 at every solver step (make_tiles), so that the memory and
+        attention cost of a step depend on the tile, not the frame.  It approximates the untiled result (GroupNorm
+        statistics, attention context and the CFG rescale become per tile) and is never switched on by itself."""
         feat = self._upload_frames(video_data_feature)
         y = y.to(self.device)
         negative_y = (self.negative_y if negative_y is None else negative_y).to(self.device)
@@ -148,6 +153,8 @@ class VideoToVideo_sr():
         chunk_inds = make_chunks(frames_num, interp_f_num=0, max_chunk_len=max_chunk_len) \
             if frames_num > max_chunk_len else None
         extra = {} if noise_sampler is None else {'noise_sampler': noise_sampler}
+        if tile_size is not None:
+            extra['tile_inds'] = make_tiles(feat.shape[3], feat.shape[4], tile_size, tile_overlap)
         model = self.generator
         if self.cuda_graph and hasattr(model, "forward_cfg_pair"):
             if self._graphed is None:
@@ -174,22 +181,25 @@ class VideoToVideo_sr():
     # -- pixel-space entry (ref :75-139) ------------------------------------------------------------
     @torch.no_grad()
     def test(self, input: Dict[str, Any], total_noise_levels=1000, steps=50, solver_mode='fast', guide_scale=7.5,
-             max_chunk_len=32):
-        """The reference entry (ref :75-139): (1, 3, F, H, W) fp32 on the CPU."""
-        return self._test_on_device(input, total_noise_levels, steps, solver_mode, guide_scale, max_chunk_len).type(torch.float32).cpu()
+             max_chunk_len=32, tile_size=None, tile_overlap=16):
+        """The reference entry (ref :75-139): (1, 3, F, H, W) fp32 on the CPU.  tile_size / tile_overlap: denoise_latents."""
+        return self._test_on_device(input, total_noise_levels, steps, solver_mode, guide_scale, max_chunk_len,
+                                    tile_size, tile_overlap).type(torch.float32).cpu()
 
     @torch.no_grad()
     def enhance_frames(self, input: Dict[str, Any], total_noise_levels=1000, steps=50, solver_mode='fast', guide_scale=7.5,
-                       max_chunk_len=32, uint8=True):
+                       max_chunk_len=32, uint8=True, tile_size=None, tile_overlap=16):
         """test() + the CLI's post-processing (inference_sr.py:77-80: tensor2vid, adain_color_fix against the LR clip) with the
         post-processing on the GPU: returns (F, H, W, 3) frames in [0, 255] on the CPU -- uint8 by default, i.e. a quarter of the
         device->host traffic of test()'s fp32 tensor."""
-        vid = self._test_on_device(input, total_noise_levels, steps, solver_mode, guide_scale, max_chunk_len).float()
+        vid = self._test_on_device(input, total_noise_levels, steps, solver_mode, guide_scale, max_chunk_len,
+                                   tile_size, tile_overlap).float()
         if vid.is_cuda:
             return ops.adain_color_fix(vid, input['video_data'].to(vid.device).float(), uint8=uint8).cpu()
         raise NotImplementedError("enhance_frames runs the GPU post-processing kernels; use test() + the reference's CPU helpers otherwise")
 
-    def _test_on_device(self, input, total_noise_levels, steps, solver_mode, guide_scale, max_chunk_len):
+    def _test_on_device(self, input, total_noise_levels, steps, solver_mode, guide_scale, max_chunk_len, tile_size=None,
+                        tile_overlap=16):
         video_data = input['video_data']
         y = input['y']
         (target_h, target_w) = input['target_res']
@@ -214,8 +224,9 @@ class VideoToVideo_sr():
         video_data_feature = feat_local if world == 1 else \
             _all_gather_varlen(feat_local.float(), [b - a for a, b in bounds], 2)
         y = self._encode_text(y)
+        tiles = {} if tile_size is None else {'tile_size': tile_size, 'tile_overlap': tile_overlap}
         gen_vid = self.denoise_latents(video_data_feature, y, None, total_noise_levels, steps, solver_mode,
-                                       guide_scale, max_chunk_len)
+                                       guide_scale, max_chunk_len, **tiles)
         logger.info('sampling, finished.')
         w1, w2, h1, h2 = padding
         with torch.autocast('cuda', enabled=torch.cuda.is_available()):
@@ -343,3 +354,48 @@ def make_chunks(f_num, interp_f_num, max_chunk_len, chunk_overlap_ratio=0.5):
     chunk_len = int((max_chunk_len - 1) // (1 + interp_f_num) * (interp_f_num + 1) + 1)
     o_len = int((max_o_len - 1) // (1 + interp_f_num) * (interp_f_num + 1) + 1)
     return sliding_windows_1d(f_num, chunk_len, o_len)
+
+
+def _tile_axis(length, tile, overlap):
+    """Tile ranges along one axis and their blend weights (fp64 ramps, normalised to a partition of unity)."""
+    if length <= tile:
+        return [(0, length)], [torch.ones(length, dtype=torch.float64)]
+    n = -(-(length - tile) // (tile - overlap)) + 1
+    starts = [k * (length - tile) // (n - 1) for k in range(n)]        # even spread: consecutive tiles overlap >= `overlap`
+    ramp = torch.arange(1, tile + 1, dtype=torch.float64) / (overlap + 1)
+    raw = []
+    for k in range(n):
+        w = torch.ones(tile, dtype=torch.float64)
+        if k > 0:                                                        # inner edges only: no ramp at the frame's border
+            w = torch.minimum(w, ramp)
+        if k < n - 1:
+            w = torch.minimum(w, ramp.flip(0))
+        raw.append(w)
+    total = torch.zeros(length, dtype=torch.float64)
+    for s, w in zip(starts, raw):
+        total[s:s + tile] += w
+    return [(s, s + tile) for s in starts], [w / total[s:s + tile] for s, w in zip(starts, raw)]
+
+
+def make_tiles(h, w, tile_size, overlap=16):
+    """Spatial tiles of an h x w latent for tiled sampling (``GaussianDiffusion.sample_sr(tile_inds=...)``).
+
+    tile_size = (th, tw) in latent units, with th = 2 (mod 8) and tw = 0 (mod 8) so that the UNet's down/up-sampling closes
+    on every tile; an axis no longer than its tile is one tile of the full extent.  Along an axis of length L > T there are
+    ceil((L - T) / (T - overlap)) + 1 tiles of size T whose starts are spread evenly over [0, L - T], so neighbours overlap
+    by at least `overlap`.  Every tile has the same shape (one CUDA graph per chunk length).
+
+    Returns (row_ranges, col_ranges, row_weights, col_weights): [(start, end)] per axis and, per tile, fp32 CPU weights of its
+    extent.  A tile's raw weight ramps linearly over `overlap` pixels up from each inner edge (none at the frame's border) and
+    is divided by the sum over all tiles covering the pixel: the weights along an axis sum to 1, a pixel covered by one tile
+    has weight exactly 1.0, and the 2-D weight of tile (i, j) at (r, c) is row_weights[i][r] * col_weights[j][c]."""
+    th, tw = (int(v) for v in tile_size)
+    if th <= 0 or tw <= 0 or th % 8 != 2 or tw % 8 != 0:
+        raise ValueError(f"tile size {th}x{tw}: the tile height must be 2 (mod 8) and the width 0 (mod 8), both positive, "
+                         "for the UNet's down/up-sampling to close")
+    overlap = int(overlap)
+    if not (0 <= overlap < min(th, tw)):
+        raise ValueError(f"tile overlap {overlap} outside [0, {min(th, tw)}) for tiles of {th}x{tw}")
+    rows, row_w = _tile_axis(int(h), th, overlap)
+    cols, col_w = _tile_axis(int(w), tw, overlap)
+    return rows, cols, [v.float() for v in row_w], [v.float() for v in col_w]
