@@ -194,68 +194,104 @@ tapgemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
         wgmma_wait<0>();
         if (prev_s >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_s]);
 
-        // ------------------------------------------------ epilogue: rows row_in_wg and row_in_wg + 8 of this warpgroup
+        // ------------------------------------------------ epilogue: rows row_in_wg and row_in_wg + 8 of this warpgroup.
+        // Per column pair the bias / colscale values are loaded once for both rows, and the residual loads of JG column
+        // pairs are issued ahead of the arithmetic that consumes them (a thread only ever stores to elements whose
+        // residual it has already read, so an output that aliases the residual stays correct).
         const int n_base = n_tile * n_per_tile;
+        bool valid[2];
+        __half* out_row[2];
+        const __half *res_row[2], *rv_row[2];
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             const int r = cw * 64 + row_in_wg + 8 * h;
             int rr = r;
             long long orow = 0, mul = 1;
-            bool valid = r < p.box_rows;
+            bool ok = r < p.box_rows;
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
                 const int l = rr % p.box[i];
                 rr /= p.box[i];
                 const int g = org[i] + l;
-                valid = valid && (g < p.on[i]);
+                ok = ok && (g < p.on[i]);
                 orow += (long long)g * mul;
                 mul *= p.on[i];
             }
-            if (!valid) continue;
-            __half* out_row = p.out + orow * p.out_ld;
-            const __half* res_row = has_res ? p.residual + orow * p.res_ld : nullptr;
-            const __half* rv_row = has_rowvec ? p.rowvec + (orow / p.rowvec_div) * p.rowvec_ld : nullptr;
+            valid[h] = ok;
+            out_row[h] = p.out + orow * p.out_ld;
+            res_row[h] = has_res ? p.residual + orow * p.res_ld : nullptr;
+            rv_row[h] = has_rowvec ? p.rowvec + (orow / p.rowvec_div) * p.rowvec_ld : nullptr;
+        }
+        if (!valid[0] && !valid[1]) continue;
+        constexpr int JG = 4;
+        constexpr int JH = BN / 16;                      // GEGLU: value column groups [0, JH), gate column groups [JH, 2 JH)
 #pragma unroll
-            for (int j = 0; j < BN / 8; ++j) {
-                if (geglu && j >= BN / 16) break;
+        for (int j0 = 0; j0 < BN / 8; j0 += JG) {
+            if (geglu && j0 >= JH) break;
+            uint32_t res2[JG][2];
+#pragma unroll
+            for (int jj = 0; jj < JG; ++jj)
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int c = 8 * (j0 + jj) + 2 * q4, n = n_base + c;
+                    res2[jj][h] = 0u;
+                    if (has_res && res_pair && valid[h] && c < n_per_tile && n + 1 < p.N)
+                        res2[jj][h] = *reinterpret_cast<const uint32_t*>(res_row[h] + n);
+                }
+#pragma unroll
+            for (int jj = 0; jj < JG; ++jj) {
+                const int j = j0 + jj;
+                const int jg = j < JH ? j + JH : j;
+                if (geglu && j >= JH) break;
                 const int c = 8 * j + 2 * q4;                    // tile column of this thread's pair
                 const int n = n_base + c;
                 if (c >= n_per_tile || n >= p.N) continue;
                 const bool two = n + 1 < p.N;
-                float f[2];
+                const int n1 = two ? n + 1 : n;                  // clamped index for the loads of a lone last column
+                float bv[2] = {0.f, 0.f}, bg[2] = {0.f, 0.f}, cs[2] = {1.f, 1.f};
+                if (has_bias) {
+                    bv[0] = tg_ld(p.bias + n);
+                    bv[1] = tg_ld(p.bias + n1);
+                    if (geglu) { bg[0] = tg_ld(p.bias + p.N + n); bg[1] = tg_ld(p.bias + p.N + n1); }
+                }
+                if (has_colscale) { cs[0] = tg_ld(p.colscale + n); cs[1] = tg_ld(p.colscale + n1); }
 #pragma unroll
-                for (int e = 0; e < 2; ++e) {
-                    float x = acc[4 * j + 2 * h + e];
-                    const int ne = (e == 1 && !two) ? n : n + e;     // clamped index for the loads of a lone last column
-                    if (geglu) {
-                        float g = acc[4 * (j + BN / 16) + 2 * h + e];
-                        if (has_bias) { x += tg_ld(p.bias + ne); g += tg_ld(p.bias + p.N + ne); }
-                        x *= gelu_erf_f(g);
-                    } else if (has_bias) {
-                        x += tg_ld(p.bias + ne);
+                for (int h = 0; h < 2; ++h) {
+                    if (!valid[h]) continue;
+                    float f[2];
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        float x = acc[4 * j + 2 * h + e];
+                        if (geglu) {
+                            float g = acc[4 * jg + 2 * h + e];
+                            if (has_bias) { x += bv[e]; g += bg[e]; }
+                            x *= gelu_erf_f(g);
+                        } else if (has_bias) {
+                            x += bv[e];
+                        }
+                        if (act_tanh) x = gelu_tanh_f(x);
+                        if (act_erf) x = gelu_erf_f(x);
+                        if (has_colscale) x *= cs[e];
+                        if (has_rowvec) x += tg_ld(rv_row[h] + (e ? n1 : n));
+                        f[e] = x;
                     }
-                    if (act_tanh) x = gelu_tanh_f(x);
-                    if (act_erf) x = gelu_erf_f(x);
-                    if (has_colscale) x *= tg_ld(p.colscale + ne);
-                    if (has_rowvec) x += tg_ld(rv_row + ne);
-                    f[e] = x;
-                }
-                if (has_res) {
-                    if (two && res_pair) {
-                        const float2 rv = __half22float2(*reinterpret_cast<const __half2*>(res_row + n));
-                        f[0] += rv.x;
-                        f[1] += rv.y;
+                    if (has_res) {
+                        if (two && res_pair) {
+                            const float2 rv = __half22float2(*reinterpret_cast<const __half2*>(&res2[jj][h]));
+                            f[0] += rv.x;
+                            f[1] += rv.y;
+                        } else {
+                            f[0] += __half2float(res_row[h][n]);
+                            if (two) f[1] += __half2float(res_row[h][n + 1]);
+                        }
+                    }
+                    if (act_silu) { f[0] = silu_f(f[0]); f[1] = silu_f(f[1]); }
+                    if (two && out_pair) {
+                        *reinterpret_cast<uint32_t*>(out_row[h] + n) = pack_half2(f[0], f[1]);
                     } else {
-                        f[0] += __half2float(res_row[n]);
-                        if (two) f[1] += __half2float(res_row[n + 1]);
+                        out_row[h][n] = __float2half_rn(f[0]);
+                        if (two) out_row[h][n + 1] = __float2half_rn(f[1]);
                     }
-                }
-                if (act_silu) { f[0] = silu_f(f[0]); f[1] = silu_f(f[1]); }
-                if (two && out_pair) {
-                    *reinterpret_cast<uint32_t*>(out_row + n) = pack_half2(f[0], f[1]);
-                } else {
-                    out_row[n] = __float2half_rn(f[0]);
-                    if (two) out_row[n + 1] = __float2half_rn(f[1]);
                 }
             }
         }
