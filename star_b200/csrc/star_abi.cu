@@ -747,7 +747,8 @@ int star_adain_color_fix(const void* video_f32, const void* source_f32, void* ou
                          long long src_hw, void* workspace, void* stream) {
     if (C < 1 || C > 4 || F < 1 || HW < 2 || src_hw < 2) return fail("star_adain_color_fix: bad geometry (C <= 4)");
     if ((out_f32 == nullptr) == (out_u8 == nullptr)) return fail("star_adain_color_fix: pass exactly one of out_f32 / out_u8");
-    if (F > 65535) return fail("star_adain_color_fix: too many frames");
+    // plane_stats_kernel runs one grid row per (channel, frame) plane: gridDim.y = C * F
+    if ((long long)C * F > 65535) return fail("star_adain_color_fix: C * F = %lld planes exceed the 65535 grid rows of the statistics launch", (long long)C * F);
     cudaStream_t st = (cudaStream_t)stream;
     double* tgt = (double*)workspace;
     double* src = tgt + (size_t)C * F * 2;

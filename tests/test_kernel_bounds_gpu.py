@@ -705,32 +705,32 @@ def test_temporal_attention_bound(ops, B, T, HW, heads, Ci, ld):
 
 
 # ---- GPU: norm statistics under a mean offset ----------------------------------------------------------------------------
-def _offset_input(rows, C, ratio, seed, per="group"):
-    """fp16 rows with unit spread around a per-group (GroupNorm) or per-row (LayerNorm) mean of +-ratio"""
+def _offset_input(rows, C, ratio, seed, per="group", dtype=HALF):
+    """fp16 (or bf16) rows with unit spread around a per-group (GroupNorm) or per-row (LayerNorm) mean of +-ratio"""
     g = torch.Generator(device="cuda").manual_seed(seed)
     if per == "group":
         mu = (ratio * (torch.randint(0, 2, (32,), generator=g, device="cuda") * 2 - 1)).repeat_interleave(C // 32)
     else:
         mu = (ratio * (torch.randint(0, 2, (rows, 1), generator=g, device="cuda") * 2 - 1))
-    x = torch.empty(rows, C, dtype=HALF, device="cuda")
+    x = torch.empty(rows, C, dtype=dtype, device="cuda")
     step = 1 << 16
     for r0 in range(0, rows, step):
         r1 = min(rows, r0 + step)
-        x[r0:r1] = (torch.randn(r1 - r0, C, generator=g, device="cuda") + (mu if per == "group" else mu[r0:r1])).half()
+        x[r0:r1] = (torch.randn(r1 - r0, C, generator=g, device="cuda") + (mu if per == "group" else mu[r0:r1])).to(dtype)
     return x
 
 
-def _norm_bound(x64, mean, rstd, gamma, beta, ymod=None, bmod=None, silu=False):
+def _norm_bound(x64, mean, rstd, gamma, beta, ymod=None, bmod=None, silu=False, dtype=HALF):
     """fp64 value and bound of y = (x - mean) rstd gamma + beta (* ymod + bmod) (SiLU)"""
     yn = (x64 - mean) * rstd
     y = yn * gamma + beta
-    err = K_STAT * U_OUT[HALF] * gamma.abs() * (yn.abs() + 1) + NORM_FP32_ROUND * U32 * (x64.abs() * rstd * gamma.abs() + beta.abs())
+    err = K_STAT * U_OUT[dtype] * gamma.abs() * (yn.abs() + 1) + NORM_FP32_ROUND * U32 * (x64.abs() * rstd * gamma.abs() + beta.abs())
     if ymod is not None:
         err = err * ymod.abs() + 2 * U32 * ((y * ymod).abs() + bmod.abs())
         y = y * ymod + bmod
     if silu:
         y, err = _silu_step(y, err)
-    return y, _finish(y, err, HALF)
+    return y, _finish(y, err, dtype)
 
 
 def _group_stats(x, ns, C, eps, step=1 << 16):

@@ -405,8 +405,9 @@ def bf16_ref():
 
 
 def test_bf16_library_kernels(env, bf16_ref):
-    """GEMM (+bias, residual, tanh-GELU, colscale), flash attention, LayerNorm, row gates, qk-LN + RoPE, SiLU on bf16 tokens
-    against the same torch references rounding to bf16 (8-bit mantissa: 8e-3 relative L2)."""
+    """GEMM (+bias, residual, tanh-GELU, colscale), flash attention, LayerNorm, the temporal row gate, SiLU, the sinusoidal
+    embedding and the spatial LIEM gate on bf16 tokens against the same torch references rounding to bf16 (8-bit mantissa:
+    8e-3 relative L2)."""
     O, R = env[0], bf16_ref
     bf = torch.bfloat16
 
