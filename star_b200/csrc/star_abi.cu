@@ -107,7 +107,7 @@ struct TapDesc {
     void* out;
 };
 
-template <int BN>
+template <int BN, int EPI>
 int launch_tapgemm_bn(const TapDesc& d, cudaStream_t st) {
     TapGemmParams p;
     memset(&p, 0, sizeof(p));
@@ -154,8 +154,30 @@ int launch_tapgemm_bn(const TapDesc& d, cudaStream_t st) {
     if (make_tmap(&tw, d.W, 2, wdim, wstr, wbox)) return 1;
 
     const int grid = (int)std::min<long long>(total, num_sms());
-    tapgemm_kernel<BN><<<grid, TG_THREADS, TapGemmSmem<BN>::TOTAL, st>>>(ta, tw, p);
+    tapgemm_kernel<BN, EPI><<<grid, TG_THREADS, TapGemmSmem<BN>::TOTAL, st>>>(ta, tw, p);
     STAR_LAUNCH_CHECK("tapgemm");
+    return 0;
+}
+
+// The epilogue instance compiled for exactly this call's epilogue kind, else the generic one.
+template <int BN>
+int launch_tapgemm_epi(const TapDesc& d, cudaStream_t st) {
+    const int kind = tg_epi_kind(d.flags, d.bias, d.rowvec, d.colscale, d.residual);
+#define TG_EPI_CASE(K)                                                                       \
+    if constexpr ((K) != TG_EPI_GENERIC && !(BN == 160 && ((K) & TG_EPI_GEGLU)))             \
+        if (kind == (K)) return launch_tapgemm_bn<BN, (K)>(d, st);
+    TG_EPI_KINDS(TG_EPI_CASE)
+#undef TG_EPI_CASE
+    return launch_tapgemm_bn<BN, TG_EPI_GENERIC>(d, st);
+}
+
+// Raises the dynamic shared-memory limit of every tile width of epilogue instance EPI.
+template <int EPI>
+int tapgemm_smem_attr() {
+    STAR_CUDA(cudaFuncSetAttribute(tapgemm_kernel<128, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, TapGemmSmem<128>::TOTAL));
+    if constexpr (EPI == TG_EPI_GENERIC || !(EPI & TG_EPI_GEGLU))
+        STAR_CUDA(cudaFuncSetAttribute(tapgemm_kernel<160, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, TapGemmSmem<160>::TOTAL));
+    STAR_CUDA(cudaFuncSetAttribute(tapgemm_kernel<256, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, TapGemmSmem<256>::TOTAL));
     return 0;
 }
 
@@ -164,11 +186,11 @@ int launch_tapgemm_bn(const TapDesc& d, cudaStream_t st) {
 int launch_tapgemm(const TapDesc& d, cudaStream_t st) {
     const bool geglu = d.flags & TG_GEGLU;
     auto padded = [&](int w) { return ((long long)d.N + w - 1) / w * w; };
-    if (geglu) return padded(128) <= padded(64) ? launch_tapgemm_bn<256>(d, st) : launch_tapgemm_bn<128>(d, st);
+    if (geglu) return padded(128) <= padded(64) ? launch_tapgemm_epi<256>(d, st) : launch_tapgemm_epi<128>(d, st);
     const long long p128 = padded(128), p160 = padded(160), p256 = padded(256);
-    if (p256 <= p128 && p256 <= p160) return launch_tapgemm_bn<256>(d, st);
-    if (p160 <= p128) return launch_tapgemm_bn<160>(d, st);
-    return launch_tapgemm_bn<128>(d, st);
+    if (p256 <= p128 && p256 <= p160) return launch_tapgemm_epi<256>(d, st);
+    if (p160 <= p128) return launch_tapgemm_epi<160>(d, st);
+    return launch_tapgemm_epi<128>(d, st);
 }
 
 void best_box_2d(int H, int W, int* th, int* tw) {
@@ -211,9 +233,10 @@ static int star_init_on_current(int device) {
         g_encode = reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(fn);
     }
 #define STAR_SMEM_ATTR(kernel, bytes) STAR_CUDA((cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(bytes))))
-    STAR_SMEM_ATTR(tapgemm_kernel<128>, TapGemmSmem<128>::TOTAL);
-    STAR_SMEM_ATTR(tapgemm_kernel<160>, TapGemmSmem<160>::TOTAL);
-    STAR_SMEM_ATTR(tapgemm_kernel<256>, TapGemmSmem<256>::TOTAL);
+#define TG_SMEM_ATTR(K) \
+    if (tapgemm_smem_attr<(K)>()) return 1;
+    TG_EPI_KINDS(TG_SMEM_ATTR)
+#undef TG_SMEM_ATTR
     STAR_SMEM_ATTR(attn_fwd_kernel, AttnSmem::TOTAL);
     STAR_SMEM_ATTR(temporal_attn2_kernel<16>, TA2_WARPS * 3 * 16 * TA2_PITCH);
     STAR_SMEM_ATTR(temporal_attn2_kernel<32>, TA2_WARPS * 3 * 32 * TA2_PITCH);

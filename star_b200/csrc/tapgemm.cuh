@@ -81,7 +81,171 @@ STAR_DEVINL void tg_mma_k16(float* acc, uint64_t da, uint64_t db) {
 
 STAR_DEVINL float tg_ld(const __half* p) { return __half2float(__ldg(p)); }
 
-template <int BN>
+// Epilogue kinds.  An instance of the kernel is compiled for one set of epilogue operations, so its unrolled
+// per-element code carries only the operations the call applies (the fully unrolled generic epilogue is 100-200 KB of
+// SASS per kernel).  TG_EPI_GENERIC reads every option from the parameters at run time: it serves any combination that
+// has no instance of its own.  The fp32 order per element is the same in every instance: bias, GEGLU / activation,
+// colscale, rowvec, residual, SiLU.
+enum TapGemmEpi : int {
+    TG_EPI_BIAS = 1,
+    TG_EPI_GEGLU = 2,
+    TG_EPI_ROWVEC = 4,
+    TG_EPI_COLSCALE = 8,
+    TG_EPI_RES = 16,
+    TG_EPI_ERF = 32,
+    TG_EPI_TANH = 64,
+    TG_EPI_SILU = 128,
+    TG_EPI_GENERIC = 256,
+};
+
+// The combinations the library's callers pass (UNet, OpenCLIP text tower, CogVideoX DiT, both VAEs), and the generic
+// instance.  Kinds with TG_EPI_GEGLU are compiled only at the tile widths GEGLU runs with (128 / 256).
+#define TG_EPI_KINDS(X)                                   \
+    X(0)                                                  \
+    X(TG_EPI_BIAS)                                        \
+    X(TG_EPI_BIAS | TG_EPI_RES)                           \
+    X(TG_EPI_BIAS | TG_EPI_ROWVEC)                        \
+    X(TG_EPI_BIAS | TG_EPI_GEGLU)                         \
+    X(TG_EPI_BIAS | TG_EPI_SILU)                          \
+    X(TG_EPI_BIAS | TG_EPI_ERF)                           \
+    X(TG_EPI_BIAS | TG_EPI_TANH)                          \
+    X(TG_EPI_BIAS | TG_EPI_COLSCALE | TG_EPI_RES)         \
+    X(TG_EPI_GENERIC)
+
+// The kind of a call: its flags and which epilogue inputs it passes.
+inline int tg_epi_kind(int flags, bool bias, bool rowvec, bool colscale, bool residual) {
+    return (bias ? TG_EPI_BIAS : 0) | ((flags & TG_GEGLU) ? TG_EPI_GEGLU : 0) | (rowvec ? TG_EPI_ROWVEC : 0) |
+           (colscale ? TG_EPI_COLSCALE : 0) | (residual ? TG_EPI_RES : 0) | ((flags & TG_GELU_ERF) ? TG_EPI_ERF : 0) |
+           ((flags & TG_GELU_TANH) ? TG_EPI_TANH : 0) | ((flags & TG_SILU_OUT) ? TG_EPI_SILU : 0);
+}
+
+// The epilogue options of instance EPI: compile-time constants, or read from the parameters for TG_EPI_GENERIC.
+template <int EPI>
+struct TapGemmEpiOpts {
+    static constexpr bool GEN = (EPI & TG_EPI_GENERIC) != 0;
+    bool geglu, bias, rowvec, colscale, res, erf, tanh, silu;
+    STAR_DEVINL explicit TapGemmEpiOpts(const TapGemmParams& p)
+        : geglu(GEN ? (p.flags & TG_GEGLU) != 0 : (EPI & TG_EPI_GEGLU) != 0),
+          bias(GEN ? p.bias != nullptr : (EPI & TG_EPI_BIAS) != 0),
+          rowvec(GEN ? p.rowvec != nullptr : (EPI & TG_EPI_ROWVEC) != 0),
+          colscale(GEN ? p.colscale != nullptr : (EPI & TG_EPI_COLSCALE) != 0),
+          res(GEN ? p.residual != nullptr : (EPI & TG_EPI_RES) != 0),
+          erf(GEN ? (p.flags & TG_GELU_ERF) != 0 : (EPI & TG_EPI_ERF) != 0),
+          tanh(GEN ? (p.flags & TG_GELU_TANH) != 0 : (EPI & TG_EPI_TANH) != 0),
+          silu(GEN ? (p.flags & TG_SILU_OUT) != 0 : (EPI & TG_EPI_SILU) != 0) {}
+};
+
+// Epilogue of one consumer warpgroup: rows row_in_wg and row_in_wg + 8 of warpgroup cw's 64 tile rows, from the
+// accumulators straight to global memory.  Per column pair the bias / colscale values are loaded once for both rows, and
+// the residual loads of JG column pairs are issued ahead of the arithmetic that consumes them (a thread only ever stores
+// to elements whose residual it has already read, so an output that aliases the residual stays correct).
+template <int BN, int EPI>
+STAR_DEVINL void tg_epilogue(const float (&acc)[BN / 2], const TapGemmParams& p, const int (&org)[4], int n_tile, int cw,
+                             int row_in_wg, int q4) {
+    const TapGemmEpiOpts<EPI> o(p);
+    const int n_per_tile = o.geglu ? BN / 2 : BN;
+    const bool out_pair = ((p.out_ld & 1) == 0) && ((reinterpret_cast<uintptr_t>(p.out) & 3) == 0);
+    const bool res_pair = !o.res || (((p.res_ld & 1) == 0) && ((reinterpret_cast<uintptr_t>(p.residual) & 3) == 0));
+    const int n_base = n_tile * n_per_tile;
+    bool valid[2];
+    __half* out_row[2];
+    const __half *res_row[2], *rv_row[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int r = cw * 64 + row_in_wg + 8 * h;
+        int rr = r;
+        long long orow = 0, mul = 1;
+        bool ok = r < p.box_rows;
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const int l = rr % p.box[i];
+            rr /= p.box[i];
+            const int g = org[i] + l;
+            ok = ok && (g < p.on[i]);
+            orow += (long long)g * mul;
+            mul *= p.on[i];
+        }
+        valid[h] = ok;
+        out_row[h] = p.out + orow * p.out_ld;
+        res_row[h] = o.res ? p.residual + orow * p.res_ld : nullptr;
+        rv_row[h] = o.rowvec ? p.rowvec + (orow / p.rowvec_div) * p.rowvec_ld : nullptr;
+    }
+    if (!valid[0] && !valid[1]) return;
+    constexpr int JG = 4;
+    constexpr int JH = BN / 16;                      // GEGLU: value column groups [0, JH), gate column groups [JH, 2 JH)
+#pragma unroll
+    for (int j0 = 0; j0 < BN / 8; j0 += JG) {
+        if (o.geglu && j0 >= JH) break;
+        uint32_t res2[JG][2];
+#pragma unroll
+        for (int jj = 0; jj < JG; ++jj)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int c = 8 * (j0 + jj) + 2 * q4, n = n_base + c;
+                res2[jj][h] = 0u;
+                if (o.res && res_pair && valid[h] && c < n_per_tile && n + 1 < p.N)
+                    res2[jj][h] = *reinterpret_cast<const uint32_t*>(res_row[h] + n);
+            }
+#pragma unroll
+        for (int jj = 0; jj < JG; ++jj) {
+            const int j = j0 + jj;
+            const int jg = j < JH ? j + JH : j;
+            if (o.geglu && j >= JH) break;
+            const int c = 8 * j + 2 * q4;                    // tile column of this thread's pair
+            const int n = n_base + c;
+            if (c >= n_per_tile || n >= p.N) continue;
+            const bool two = n + 1 < p.N;
+            const int n1 = two ? n + 1 : n;                  // clamped index for the loads of a lone last column
+            float bv[2] = {0.f, 0.f}, bg[2] = {0.f, 0.f}, cs[2] = {1.f, 1.f};
+            if (o.bias) {
+                bv[0] = tg_ld(p.bias + n);
+                bv[1] = tg_ld(p.bias + n1);
+                if (o.geglu) { bg[0] = tg_ld(p.bias + p.N + n); bg[1] = tg_ld(p.bias + p.N + n1); }
+            }
+            if (o.colscale) { cs[0] = tg_ld(p.colscale + n); cs[1] = tg_ld(p.colscale + n1); }
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                if (!valid[h]) continue;
+                float f[2];
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    float x = acc[4 * j + 2 * h + e];
+                    if (o.geglu) {
+                        float g = acc[4 * jg + 2 * h + e];
+                        if (o.bias) { x += bv[e]; g += bg[e]; }
+                        x *= gelu_erf_f(g);
+                    } else if (o.bias) {
+                        x += bv[e];
+                    }
+                    if (o.tanh) x = gelu_tanh_f(x);
+                    if (o.erf) x = gelu_erf_f(x);
+                    if (o.colscale) x *= cs[e];
+                    if (o.rowvec) x += tg_ld(rv_row[h] + (e ? n1 : n));
+                    f[e] = x;
+                }
+                if (o.res) {
+                    if (two && res_pair) {
+                        const float2 rv = __half22float2(*reinterpret_cast<const __half2*>(&res2[jj][h]));
+                        f[0] += rv.x;
+                        f[1] += rv.y;
+                    } else {
+                        f[0] += __half2float(res_row[h][n]);
+                        if (two) f[1] += __half2float(res_row[h][n + 1]);
+                    }
+                }
+                if (o.silu) { f[0] = silu_f(f[0]); f[1] = silu_f(f[1]); }
+                if (two && out_pair) {
+                    *reinterpret_cast<uint32_t*>(out_row[h] + n) = pack_half2(f[0], f[1]);
+                } else {
+                    out_row[h][n] = __float2half_rn(f[0]);
+                    if (two) out_row[h][n + 1] = __float2half_rn(f[1]);
+                }
+            }
+        }
+    }
+}
+
+template <int BN, int EPI>
 __global__ void __launch_bounds__(TG_THREADS, 1)
 tapgemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_w,
                const __grid_constant__ TapGemmParams p) {
@@ -95,8 +259,7 @@ tapgemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
     const int wg = threadIdx.x >> 7;
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
-    const bool geglu = (p.flags & TG_GEGLU) != 0;
-    const int n_per_tile = geglu ? BN / 2 : BN;      // output columns produced per tile
+    const bool geglu = TapGemmEpiOpts<EPI>(p).geglu;
     const int total_iters = p.ntaps * p.k_chunks;
 
     if (threadIdx.x == 0) {
@@ -162,12 +325,6 @@ tapgemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
     const uint64_t desc_a0 = wgmma_desc_sw128(smem_u32(smem) + cw * 64 * 128, 16, 1024);
     const uint64_t desc_b0 = wgmma_desc_sw128(smem_u32(smem) + SM::A_BYTES, 16, 1024);
     constexpr uint64_t STAGE_INC = (uint64_t)(SM::STAGE_BYTES >> 4);
-    const bool has_bias = p.bias != nullptr, has_rowvec = p.rowvec != nullptr, has_colscale = p.colscale != nullptr;
-    const bool has_res = p.residual != nullptr;
-    const bool act_tanh = (p.flags & TG_GELU_TANH) != 0, act_erf = (p.flags & TG_GELU_ERF) != 0;
-    const bool act_silu = (p.flags & TG_SILU_OUT) != 0;
-    const bool out_pair = ((p.out_ld & 1) == 0) && ((reinterpret_cast<uintptr_t>(p.out) & 3) == 0);
-    const bool res_pair = !has_res || (((p.res_ld & 1) == 0) && ((reinterpret_cast<uintptr_t>(p.residual) & 3) == 0));
     int s = 0;
     uint32_t ph = 0;
     for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
@@ -194,107 +351,7 @@ tapgemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
         wgmma_wait<0>();
         if (prev_s >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_s]);
 
-        // ------------------------------------------------ epilogue: rows row_in_wg and row_in_wg + 8 of this warpgroup.
-        // Per column pair the bias / colscale values are loaded once for both rows, and the residual loads of JG column
-        // pairs are issued ahead of the arithmetic that consumes them (a thread only ever stores to elements whose
-        // residual it has already read, so an output that aliases the residual stays correct).
-        const int n_base = n_tile * n_per_tile;
-        bool valid[2];
-        __half* out_row[2];
-        const __half *res_row[2], *rv_row[2];
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-            const int r = cw * 64 + row_in_wg + 8 * h;
-            int rr = r;
-            long long orow = 0, mul = 1;
-            bool ok = r < p.box_rows;
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const int l = rr % p.box[i];
-                rr /= p.box[i];
-                const int g = org[i] + l;
-                ok = ok && (g < p.on[i]);
-                orow += (long long)g * mul;
-                mul *= p.on[i];
-            }
-            valid[h] = ok;
-            out_row[h] = p.out + orow * p.out_ld;
-            res_row[h] = has_res ? p.residual + orow * p.res_ld : nullptr;
-            rv_row[h] = has_rowvec ? p.rowvec + (orow / p.rowvec_div) * p.rowvec_ld : nullptr;
-        }
-        if (!valid[0] && !valid[1]) continue;
-        constexpr int JG = 4;
-        constexpr int JH = BN / 16;                      // GEGLU: value column groups [0, JH), gate column groups [JH, 2 JH)
-#pragma unroll
-        for (int j0 = 0; j0 < BN / 8; j0 += JG) {
-            if (geglu && j0 >= JH) break;
-            uint32_t res2[JG][2];
-#pragma unroll
-            for (int jj = 0; jj < JG; ++jj)
-#pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    const int c = 8 * (j0 + jj) + 2 * q4, n = n_base + c;
-                    res2[jj][h] = 0u;
-                    if (has_res && res_pair && valid[h] && c < n_per_tile && n + 1 < p.N)
-                        res2[jj][h] = *reinterpret_cast<const uint32_t*>(res_row[h] + n);
-                }
-#pragma unroll
-            for (int jj = 0; jj < JG; ++jj) {
-                const int j = j0 + jj;
-                const int jg = j < JH ? j + JH : j;
-                if (geglu && j >= JH) break;
-                const int c = 8 * j + 2 * q4;                    // tile column of this thread's pair
-                const int n = n_base + c;
-                if (c >= n_per_tile || n >= p.N) continue;
-                const bool two = n + 1 < p.N;
-                const int n1 = two ? n + 1 : n;                  // clamped index for the loads of a lone last column
-                float bv[2] = {0.f, 0.f}, bg[2] = {0.f, 0.f}, cs[2] = {1.f, 1.f};
-                if (has_bias) {
-                    bv[0] = tg_ld(p.bias + n);
-                    bv[1] = tg_ld(p.bias + n1);
-                    if (geglu) { bg[0] = tg_ld(p.bias + p.N + n); bg[1] = tg_ld(p.bias + p.N + n1); }
-                }
-                if (has_colscale) { cs[0] = tg_ld(p.colscale + n); cs[1] = tg_ld(p.colscale + n1); }
-#pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    if (!valid[h]) continue;
-                    float f[2];
-#pragma unroll
-                    for (int e = 0; e < 2; ++e) {
-                        float x = acc[4 * j + 2 * h + e];
-                        if (geglu) {
-                            float g = acc[4 * jg + 2 * h + e];
-                            if (has_bias) { x += bv[e]; g += bg[e]; }
-                            x *= gelu_erf_f(g);
-                        } else if (has_bias) {
-                            x += bv[e];
-                        }
-                        if (act_tanh) x = gelu_tanh_f(x);
-                        if (act_erf) x = gelu_erf_f(x);
-                        if (has_colscale) x *= cs[e];
-                        if (has_rowvec) x += tg_ld(rv_row[h] + (e ? n1 : n));
-                        f[e] = x;
-                    }
-                    if (has_res) {
-                        if (two && res_pair) {
-                            const float2 rv = __half22float2(*reinterpret_cast<const __half2*>(&res2[jj][h]));
-                            f[0] += rv.x;
-                            f[1] += rv.y;
-                        } else {
-                            f[0] += __half2float(res_row[h][n]);
-                            if (two) f[1] += __half2float(res_row[h][n + 1]);
-                        }
-                    }
-                    if (act_silu) { f[0] = silu_f(f[0]); f[1] = silu_f(f[1]); }
-                    if (two && out_pair) {
-                        *reinterpret_cast<uint32_t*>(out_row[h] + n) = pack_half2(f[0], f[1]);
-                    } else {
-                        out_row[h][n] = __float2half_rn(f[0]);
-                        if (two) out_row[h][n + 1] = __float2half_rn(f[1]);
-                    }
-                }
-            }
-        }
+        tg_epilogue<BN, EPI>(acc, p, org, n_tile, cw, row_in_wg, q4);
     }
 }
 

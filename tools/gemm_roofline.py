@@ -44,6 +44,25 @@ def tile_width(n, geglu):
     return 160 if pad(160) <= pad(128) else 128
 
 
+# epilogue instances (tapgemm.cuh: TapGemmEpi, TG_EPI_KINDS, tg_epi_kind): a call runs the instance compiled for exactly its
+# epilogue kind, else the generic one that reads every option at run time
+EPI_BITS = {"bias": 1, "geglu": 2, "rowvec": 4, "colscale": 8, "residual": 16, "erf": 32, "tanh": 64, "silu": 128}
+EPI_GENERIC = 256
+EPI_INSTANCES = (0, 1, 1 | 16, 1 | 4, 1 | 2, 1 | 128, 1 | 32, 1 | 64, 1 | 8 | 16)
+
+
+def epi_kind(flags, epi):
+    """tg_epi_kind: the epilogue kind of a call from its flags and the epilogue inputs it passes"""
+    names = set(epi) | {n for bit, n in ((1, "geglu"), (2, "silu"), (4, "erf"), (8, "tanh")) if flags & bit}
+    return sum(EPI_BITS[n] for n in names)
+
+
+def epi_instance(flags, epi):
+    """the epilogue instance a call runs: its own kind's, or EPI_GENERIC"""
+    k = epi_kind(flags, epi)
+    return k if k in EPI_INSTANCES else EPI_GENERIC
+
+
 def best_box_2d(h, w):
     best, th, tw = -1, 1, 1
     for bw in range(1, min(w, 128) + 1):
@@ -153,7 +172,8 @@ def model(shape, sms=NUM_SMS):
     return {"M": M, "N": N, "K": K, "taps": taps, "bn": bn, "tiles": tiles, "waves": tiles / sms, "iters": iters,
             "geglu": geglu, "flops": flops, "hbm_bytes": hbm, "fill_bytes": fill, "mma_floor_ms": t_mma, "hbm_floor_ms": t_hbm,
             "floor_ms": max(t_mma, t_hbm), "bound": "MMA" if t_mma >= t_hbm else "HBM",
-            "fill_needed_b_clk_sm": fill / (flops / 4096.0)}      # at 2048 dense fp16 FMA per clock per SM
+            "fill_needed_b_clk_sm": fill / (flops / 4096.0),      # at 2048 dense fp16 FMA per clock per SM
+            "epi_instance": epi_instance(shape.flags, shape.epi)}
 
 
 def label(shape):
@@ -323,7 +343,7 @@ def main():
                "fill_b_clk_sm": m["fill_bytes"] / (ms * 1e-3 * mhz * 1e6 * sms) if mhz else float("nan"),
                "share_of_gemm": ms * c / gemm_step if gemm_step else None, "in_step_ms": in_step.get(s),
                **{k: m[k] for k in ("M", "N", "K", "taps", "bn", "tiles", "waves", "flops", "hbm_bytes", "fill_bytes", "hbm_floor_ms",
-                                    "mma_floor_ms", "bound", "fill_needed_b_clk_sm")}}
+                                    "mma_floor_ms", "bound", "fill_needed_b_clk_sm", "epi_instance")}}
         rows.append(row)
         print(f"{('sweep ' if row['sweep'] else '') + row['shape']:58s} {c:5d} {m['bn']:3d} {m['waves']:6.1f} {ms:8.3f} "
               f"{row['tflops']:8.1f} {m['hbm_floor_ms']:7.3f} {m['mma_floor_ms']:7.3f} {m['bound']:>5s} {ms / m['floor_ms']:7.2f} "
