@@ -8,7 +8,6 @@
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
-#include <cstring>
 #include <string>
 
 #include "../../include/star_sm100.h"
@@ -93,118 +92,96 @@ inline int grid_for(long long n, int block, int cap_mult = 32) {
 }
 
 // ------------------------------------------------------------------ tap-GEMM launcher
-struct TapDesc {
-    const void* A;
-    unsigned long long adim[5];      // (C, n1..n4) of the input view
-    unsigned long long astr[5];      // element strides of dims 1..4 (astr[0] unused)
-    int on[4];                       // output extents
-    int box[4];
-    int ntaps;
-    int tap[TG_MAX_TAPS][4];
-    int K, N, flags;
-    const void *W, *bias, *rowvec, *residual, *colscale;
-    long long rowvec_div, ldrowvec, ldres, ldo;
-    void* out;
-};
+// Tile width: the one of 128 / 160 / 256 output columns (GEGLU: 64 / 128 value columns) that pads N least, the wider on
+// a tie (fewer tiles, more reuse of each A tile).
+int tile_width(int N, bool geglu) {
+    auto padded = [&](int w) { return ((long long)N + w - 1) / w * w; };
+    if (geglu) return padded(128) <= padded(64) ? 256 : 128;
+    const long long p128 = padded(128), p160 = padded(160), p256 = padded(256);
+    if (p256 <= p128 && p256 <= p160) return 256;
+    return p160 <= p128 ? 160 : 128;
+}
 
+// The epilogue instance compiled for exactly this call's epilogue kind, else the generic one.
+template <int BN>
+void launch_tapgemm_epi(const CUtensorMap& ta, const CUtensorMap& tw, const TapGemmParams& p, int grid, cudaStream_t st) {
+    const int kind = tg_epi_kind(p.flags, p.bias, p.rowvec, p.colscale, p.residual);
+    auto kernel = tapgemm_kernel<BN, TG_EPI_GENERIC>;
+#define TG_EPI_CASE(K)                                                     \
+    if constexpr ((K) != TG_EPI_GENERIC && tg_instance(BN, (K)))          \
+        if (kind == (K)) kernel = tapgemm_kernel<BN, (K)>;
+    TG_EPI_KINDS(TG_EPI_CASE)
+#undef TG_EPI_CASE
+    kernel<<<grid, TG_THREADS, TapGemmSmem<BN>::TOTAL, st>>>(ta, tw, p);
+}
+
+// Raises the dynamic shared-memory limit of instance <BN, EPI>, if it is compiled.
 template <int BN, int EPI>
-int launch_tapgemm_bn(const TapDesc& d, cudaStream_t st) {
-    TapGemmParams p;
-    memset(&p, 0, sizeof(p));
+int tapgemm_smem_attr() {
+    if constexpr (tg_instance(BN, EPI))
+        STAR_CUDA(cudaFuncSetAttribute(tapgemm_kernel<BN, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, TapGemmSmem<BN>::TOTAL));
+    return 0;
+}
+
+// Launches a tap-GEMM whose caller has filled p's output extents, box, taps, K, N, flags and epilogue inputs.  A holds
+// p.K channels per row, rows lda elements apart, viewed as extents n1..n4 (n1 fastest); W is [N (2N with GEGLU), ntaps * K].
+// Every other field of p, and both tensor maps, follow from those here.
+int launch_tapgemm(TapGemmParams& p, const void* A, unsigned long long lda, unsigned long long n1, unsigned long long n2,
+                   unsigned long long n3, unsigned long long n4, const void* W, cudaStream_t st) {
     long long m_tiles = 1;
-    int box_rows = 1;
+    p.box_rows = 1;
     for (int i = 0; i < 4; ++i) {
-        p.on[i] = d.on[i];
-        p.box[i] = d.box[i];
-        p.tiles[i] = (d.on[i] + d.box[i] - 1) / d.box[i];
+        p.tiles[i] = (p.on[i] + p.box[i] - 1) / p.box[i];
         m_tiles *= p.tiles[i];
-        box_rows *= d.box[i];
+        p.box_rows *= p.box[i];
     }
-    if (box_rows > TG_BM) return fail("tapgemm: box has %d rows (> %d)", box_rows, TG_BM);
-    p.box_rows = box_rows;
-    p.ntaps = d.ntaps;
-    memcpy(p.tap, d.tap, sizeof(p.tap));
-    p.K = d.K;
-    p.k_chunks = (d.K + TG_BK - 1) / TG_BK;
-    p.N = d.N;
-    p.flags = d.flags;
-    p.bias = (const __half*)d.bias;
-    p.rowvec = (const __half*)d.rowvec;
-    p.rowvec_div = (int)std::max(1ll, d.rowvec_div);
-    p.rowvec_ld = d.ldrowvec > 0 ? d.ldrowvec : d.N;
-    p.residual = (const __half*)d.residual;
-    p.colscale = (const __half*)d.colscale;
-    p.res_ld = d.ldres;
-    p.out = (__half*)d.out;
-    p.out_ld = d.ldo;
-    const bool geglu = d.flags & TG_GEGLU;
-    const int n_per_tile = geglu ? BN / 2 : BN;
-    p.n_tiles = (d.N + n_per_tile - 1) / n_per_tile;
+    if (p.box_rows > TG_BM) return fail("tapgemm: box has %d rows (> %d)", p.box_rows, TG_BM);
+    p.k_chunks = (p.K + TG_BK - 1) / TG_BK;
+    p.rowvec_div = std::max(1, p.rowvec_div);
+    if (p.rowvec_ld <= 0) p.rowvec_ld = p.N;
+    const bool geglu = p.flags & TG_GEGLU;
+    const int bn = tile_width(p.N, geglu);
+    const int n_per_tile = geglu ? bn / 2 : bn;
+    p.n_tiles = (p.N + n_per_tile - 1) / n_per_tile;
     const long long total = m_tiles * p.n_tiles;
     if (total > 0x7fffffffll) return fail("tapgemm: too many tiles");
     p.num_tiles = (int)total;
 
     CUtensorMap ta, tw;
-    unsigned abox[5] = {TG_BK, (unsigned)d.box[0], (unsigned)d.box[1], (unsigned)d.box[2], (unsigned)d.box[3]};
-    if (make_tmap(&ta, d.A, 5, d.adim, d.astr, abox)) return 1;
-    const unsigned long long wrows = geglu ? 2ull * d.N : (unsigned long long)d.N;
-    unsigned long long wdim[2] = {(unsigned long long)d.ntaps * d.K, wrows};
-    unsigned long long wstr[2] = {1, (unsigned long long)d.ntaps * d.K};
+    unsigned long long adim[5] = {(unsigned long long)p.K, n1, n2, n3, n4}, astr[5] = {1, lda};
+    for (int i = 2; i < 5; ++i) astr[i] = astr[i - 1] * adim[i - 1];
+    unsigned abox[5] = {TG_BK, (unsigned)p.box[0], (unsigned)p.box[1], (unsigned)p.box[2], (unsigned)p.box[3]};
+    if (make_tmap(&ta, A, 5, adim, astr, abox)) return 1;
+    const unsigned long long wrows = geglu ? 2ull * p.N : (unsigned long long)p.N;
+    unsigned long long wdim[2] = {(unsigned long long)p.ntaps * p.K, wrows};
+    unsigned long long wstr[2] = {1, (unsigned long long)p.ntaps * p.K};
     unsigned wbox[2] = {TG_BK, (unsigned)n_per_tile};
-    if (make_tmap(&tw, d.W, 2, wdim, wstr, wbox)) return 1;
+    if (make_tmap(&tw, W, 2, wdim, wstr, wbox)) return 1;
 
     const int grid = (int)std::min<long long>(total, num_sms());
-    tapgemm_kernel<BN, EPI><<<grid, TG_THREADS, TapGemmSmem<BN>::TOTAL, st>>>(ta, tw, p);
+    if (bn == 256) launch_tapgemm_epi<256>(ta, tw, p, grid, st);
+    else if (bn == 160) launch_tapgemm_epi<160>(ta, tw, p, grid, st);
+    else launch_tapgemm_epi<128>(ta, tw, p, grid, st);
     STAR_LAUNCH_CHECK("tapgemm");
     return 0;
 }
 
-// The epilogue instance compiled for exactly this call's epilogue kind, else the generic one.
-template <int BN>
-int launch_tapgemm_epi(const TapDesc& d, cudaStream_t st) {
-    const int kind = tg_epi_kind(d.flags, d.bias, d.rowvec, d.colscale, d.residual);
-#define TG_EPI_CASE(K)                                                                       \
-    if constexpr ((K) != TG_EPI_GENERIC && !(BN == 160 && ((K) & TG_EPI_GEGLU)))             \
-        if (kind == (K)) return launch_tapgemm_bn<BN, (K)>(d, st);
-    TG_EPI_KINDS(TG_EPI_CASE)
-#undef TG_EPI_CASE
-    return launch_tapgemm_bn<BN, TG_EPI_GENERIC>(d, st);
-}
-
-// Raises the dynamic shared-memory limit of every tile width of epilogue instance EPI.
-template <int EPI>
-int tapgemm_smem_attr() {
-    STAR_CUDA(cudaFuncSetAttribute(tapgemm_kernel<128, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, TapGemmSmem<128>::TOTAL));
-    if constexpr (EPI == TG_EPI_GENERIC || !(EPI & TG_EPI_GEGLU))
-        STAR_CUDA(cudaFuncSetAttribute(tapgemm_kernel<160, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, TapGemmSmem<160>::TOTAL));
-    STAR_CUDA(cudaFuncSetAttribute(tapgemm_kernel<256, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, TapGemmSmem<256>::TOTAL));
-    return 0;
-}
-
-// Tile width: the one of 128 / 160 / 256 output columns (GEGLU: 64 / 128 value columns) that pads N least, the wider on
-// a tie (fewer tiles, more reuse of each A tile).
-int launch_tapgemm(const TapDesc& d, cudaStream_t st) {
-    const bool geglu = d.flags & TG_GEGLU;
-    auto padded = [&](int w) { return ((long long)d.N + w - 1) / w * w; };
-    if (geglu) return padded(128) <= padded(64) ? launch_tapgemm_epi<256>(d, st) : launch_tapgemm_epi<128>(d, st);
-    const long long p128 = padded(128), p160 = padded(160), p256 = padded(256);
-    if (p256 <= p128 && p256 <= p160) return launch_tapgemm_epi<256>(d, st);
-    if (p160 <= p128) return launch_tapgemm_epi<160>(d, st);
-    return launch_tapgemm_epi<128>(d, st);
-}
-
-void best_box_2d(int H, int W, int* th, int* tw) {
+// Box of a conv tile over (w, h, frames): the 2-D box of at most 128 pixels that covers H x W in the fewest tiles (the
+// wider on a tie), then as many of `frames` frames as fill 128 rows.
+void conv_box(int H, int W, int frames, int* box) {
     long long best = -1;
+    int th = 1, tw = 1;
     for (int w = 1; w <= std::min(W, 128); ++w) {
         int h = std::min(H, 128 / w);
         if (h < 1) continue;
         long long tiles = (long long)((W + w - 1) / w) * ((H + h - 1) / h);
-        if (best < 0 || tiles < best || (tiles == best && w > *tw)) {
+        if (best < 0 || tiles < best || (tiles == best && w > tw)) {
             best = tiles;
-            *th = h;
-            *tw = w;
+            th = h;
+            tw = w;
         }
     }
+    box[0] = tw; box[1] = th; box[2] = std::max(1, std::min(frames, TG_BM / (tw * th))); box[3] = 1;
 }
 
 }  // namespace
@@ -234,7 +211,7 @@ static int star_init_on_current(int device) {
     }
 #define STAR_SMEM_ATTR(kernel, bytes) STAR_CUDA((cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(bytes))))
 #define TG_SMEM_ATTR(K) \
-    if (tapgemm_smem_attr<(K)>()) return 1;
+    if (tapgemm_smem_attr<128, (K)>() || tapgemm_smem_attr<160, (K)>() || tapgemm_smem_attr<256, (K)>()) return 1;
     TG_EPI_KINDS(TG_SMEM_ATTR)
 #undef TG_SMEM_ATTR
     STAR_SMEM_ATTR(attn_fwd_kernel, AttnSmem::TOTAL);
@@ -271,20 +248,16 @@ int star_linear_ex(const void* A, long long lda, const void* W, const void* bias
     STAR_CHECK_INIT();
     if (rows <= 0) return 0;
     if (K % 8 || lda % 8) return fail("star_linear: K and lda must be multiples of 8 (K=%d lda=%lld)", K, lda);
-    TapDesc d;
-    memset(&d, 0, sizeof(d));
-    d.A = A;
-    d.adim[0] = K; d.adim[1] = rows; d.adim[2] = d.adim[3] = d.adim[4] = 1;
-    d.astr[1] = lda; d.astr[2] = d.astr[3] = d.astr[4] = (unsigned long long)lda * rows;
-    d.on[0] = (int)rows; d.on[1] = d.on[2] = d.on[3] = 1;
-    d.box[0] = TG_BM; d.box[1] = d.box[2] = d.box[3] = 1;
     if (rows > 0x7fffffffll) return fail("star_linear: too many rows");
-    d.ntaps = 1;
-    d.K = K; d.N = N; d.flags = flags;
-    d.W = W; d.bias = bias; d.rowvec = rowvec; d.rowvec_div = rowvec_div; d.residual = residual; d.ldres = ldres;
-    d.colscale = colscale;
-    d.out = out; d.ldo = ldo;
-    return launch_tapgemm(d, (cudaStream_t)stream);
+    TapGemmParams p{};
+    p.on[0] = (int)rows; p.on[1] = p.on[2] = p.on[3] = 1;
+    p.box[0] = TG_BM; p.box[1] = p.box[2] = p.box[3] = 1;
+    p.ntaps = 1;
+    p.K = K; p.N = N; p.flags = flags;
+    p.bias = (const __half*)bias; p.rowvec = (const __half*)rowvec; p.rowvec_div = (int)rowvec_div;
+    p.colscale = (const __half*)colscale; p.residual = (const __half*)residual; p.res_ld = ldres;
+    p.out = (__half*)out; p.out_ld = ldo;
+    return launch_tapgemm(p, A, lda, rows, 1, 1, 1, W, (cudaStream_t)stream);
 }
 
 int star_conv2d_3x3(const void* X, const void* W9, const void* bias, const void* rowvec, long long rowvec_div, long long ldrowvec,
@@ -292,27 +265,21 @@ int star_conv2d_3x3(const void* X, const void* W9, const void* bias, const void*
                     int Cout, void* stream) {
     STAR_CHECK_INIT();
     if (Cin % 8) return fail("star_conv2d_3x3: Cin must be a multiple of 8");
-    TapDesc d;
-    memset(&d, 0, sizeof(d));
-    d.A = X;
-    d.adim[0] = Cin; d.adim[1] = W; d.adim[2] = H; d.adim[3] = BT; d.adim[4] = 1;
-    d.astr[1] = Cin; d.astr[2] = (unsigned long long)Cin * W; d.astr[3] = (unsigned long long)Cin * W * H;
-    d.astr[4] = (unsigned long long)Cin * W * H * BT;
-    d.on[0] = W; d.on[1] = H; d.on[2] = BT; d.on[3] = 1;
-    int th = 1, tw = 1;
-    best_box_2d(H, W, &th, &tw);
-    d.box[0] = tw; d.box[1] = th; d.box[2] = std::max(1, std::min(BT, TG_BM / (tw * th))); d.box[3] = 1;
-    d.ntaps = 9;
+    if (rowvec && ldrowvec % 8) return fail("star_conv2d_3x3: ldrowvec must be a multiple of 8");
+    TapGemmParams p{};
+    p.on[0] = W; p.on[1] = H; p.on[2] = BT; p.on[3] = 1;
+    conv_box(H, W, BT, p.box);
+    p.ntaps = 9;
     for (int r = 0; r < 3; ++r)
         for (int s = 0; s < 3; ++s) {
-            d.tap[r * 3 + s][0] = s - 1;
-            d.tap[r * 3 + s][1] = r - 1;
+            p.tap[r * 3 + s][0] = s - 1;
+            p.tap[r * 3 + s][1] = r - 1;
         }
-    d.K = Cin; d.N = Cout;
-    d.W = W9; d.bias = bias; d.rowvec = rowvec; d.rowvec_div = rowvec_div; d.ldrowvec = ldrowvec; d.residual = residual; d.ldres = ldres;
-    if (rowvec && ldrowvec % 8) return fail("star_conv2d_3x3: ldrowvec must be a multiple of 8");
-    d.out = out; d.ldo = ldo;
-    return launch_tapgemm(d, (cudaStream_t)stream);
+    p.K = Cin; p.N = Cout;
+    p.bias = (const __half*)bias; p.rowvec = (const __half*)rowvec; p.rowvec_div = (int)rowvec_div; p.rowvec_ld = ldrowvec;
+    p.residual = (const __half*)residual; p.res_ld = ldres;
+    p.out = (__half*)out; p.out_ld = ldo;
+    return launch_tapgemm(p, X, Cin, W, H, BT, 1, W9, (cudaStream_t)stream);
 }
 
 long long star_conv2d_s2p_workspace_bytes(int BT, int H, int W, int Cin, int pad_t, int pad_b, int pad_l, int pad_r) {
@@ -341,27 +308,20 @@ int star_conv2d_3x3_s2p(const void* X, const void* W9, const void* bias, void* o
     const long long n = (long long)BT * 4 * H2 * W2 * (Cin / 8);
     s2_split_kernel<<<grid_for(n, 256), 256, 0, st>>>((const __half*)X, (__half*)planes_ws, BT, H, W, Cin, H2, W2, pad_t, pad_l);
     STAR_LAUNCH_CHECK("s2_split");
-    TapDesc d;
-    memset(&d, 0, sizeof(d));
-    d.A = planes_ws;
-    d.adim[0] = Cin; d.adim[1] = W2; d.adim[2] = H2; d.adim[3] = 4; d.adim[4] = BT;
-    d.astr[1] = Cin; d.astr[2] = (unsigned long long)Cin * W2; d.astr[3] = (unsigned long long)Cin * W2 * H2;
-    d.astr[4] = (unsigned long long)Cin * W2 * H2 * 4;
-    d.on[0] = Wo; d.on[1] = Ho; d.on[2] = 1; d.on[3] = BT;
-    int th = 1, tw = 1;
-    best_box_2d(Ho, Wo, &th, &tw);
-    d.box[0] = tw; d.box[1] = th; d.box[2] = 1; d.box[3] = 1;
-    d.ntaps = 9;
+    TapGemmParams p{};
+    p.on[0] = Wo; p.on[1] = Ho; p.on[2] = 1; p.on[3] = BT;
+    conv_box(Ho, Wo, 1, p.box);
+    p.ntaps = 9;
     for (int r = 0; r < 3; ++r)
         for (int s = 0; s < 3; ++s) {
-            d.tap[r * 3 + s][0] = s >> 1;
-            d.tap[r * 3 + s][1] = r >> 1;
-            d.tap[r * 3 + s][2] = (r & 1) * 2 + (s & 1);
+            p.tap[r * 3 + s][0] = s >> 1;
+            p.tap[r * 3 + s][1] = r >> 1;
+            p.tap[r * 3 + s][2] = (r & 1) * 2 + (s & 1);
         }
-    d.K = Cin; d.N = Cout;
-    d.W = W9; d.bias = bias;
-    d.out = out; d.ldo = ldo;
-    return launch_tapgemm(d, st);
+    p.K = Cin; p.N = Cout;
+    p.bias = (const __half*)bias;
+    p.out = (__half*)out; p.out_ld = ldo;
+    return launch_tapgemm(p, planes_ws, Cin, W2, H2, 4, BT, W9, st);
 }
 
 int star_conv_t3(const void* X, const void* W3, const void* bias, const void* residual, long long ldres, void* out,
@@ -369,21 +329,16 @@ int star_conv_t3(const void* X, const void* W3, const void* bias, const void* re
     STAR_CHECK_INIT();
     if (Cin % 8) return fail("star_conv_t3: Cin must be a multiple of 8");
     if (HW > 0x7fffffffll) return fail("star_conv_t3: HW too large");
-    TapDesc d;
-    memset(&d, 0, sizeof(d));
-    d.A = X;
-    d.adim[0] = Cin; d.adim[1] = HW; d.adim[2] = T; d.adim[3] = B; d.adim[4] = 1;
-    d.astr[1] = Cin; d.astr[2] = (unsigned long long)Cin * HW; d.astr[3] = (unsigned long long)Cin * HW * T;
-    d.astr[4] = (unsigned long long)Cin * HW * T * B;
-    d.on[0] = (int)HW; d.on[1] = T; d.on[2] = B; d.on[3] = 1;
-    d.box[0] = (int)std::min<long long>(TG_BM, HW); d.box[1] = 1; d.box[2] = 1; d.box[3] = 1;
-    if (HW < TG_BM) d.box[1] = (int)std::min<long long>(T, TG_BM / HW);     // small latents: several frames per tile
-    d.ntaps = 3;
-    for (int k = 0; k < 3; ++k) d.tap[k][1] = k - 1;
-    d.K = Cin; d.N = Cout;
-    d.W = W3; d.bias = bias; d.residual = residual; d.ldres = ldres;
-    d.out = out; d.ldo = ldo;
-    return launch_tapgemm(d, (cudaStream_t)stream);
+    TapGemmParams p{};
+    p.on[0] = (int)HW; p.on[1] = T; p.on[2] = B; p.on[3] = 1;
+    p.box[0] = (int)std::min<long long>(TG_BM, HW); p.box[1] = 1; p.box[2] = 1; p.box[3] = 1;
+    if (HW < TG_BM) p.box[1] = (int)std::min<long long>(T, TG_BM / HW);     // small latents: several frames per tile
+    p.ntaps = 3;
+    for (int k = 0; k < 3; ++k) p.tap[k][1] = k - 1;
+    p.K = Cin; p.N = Cout;
+    p.bias = (const __half*)bias; p.residual = (const __half*)residual; p.res_ld = ldres;
+    p.out = (__half*)out; p.out_ld = ldo;
+    return launch_tapgemm(p, X, Cin, HW, T, B, 1, W3, (cudaStream_t)stream);
 }
 
 // Causal Conv3d 3x3x3 of the CogVideoX 3-D VAE (cogvideox-based/sat/vae_modules/cp_enc_dec.py:360-430): X holds T + 2 frames --
@@ -394,27 +349,20 @@ int star_conv3d_causal(const void* X, const void* W27, const void* bias, const v
                        long long ldo, int T, int H, int W, int Cin, int Cout, void* stream) {
     STAR_CHECK_INIT();
     if (Cin % 8) return fail("star_conv3d_causal: Cin must be a multiple of 8");
-    TapDesc d;
-    memset(&d, 0, sizeof(d));
-    d.A = X;
-    d.adim[0] = Cin; d.adim[1] = W; d.adim[2] = H; d.adim[3] = T + 2; d.adim[4] = 1;
-    d.astr[1] = Cin; d.astr[2] = (unsigned long long)Cin * W; d.astr[3] = (unsigned long long)Cin * W * H;
-    d.astr[4] = (unsigned long long)Cin * W * H * (T + 2);
-    d.on[0] = W; d.on[1] = H; d.on[2] = T; d.on[3] = 1;
-    int th = 1, tw = 1;
-    best_box_2d(H, W, &th, &tw);
-    d.box[0] = tw; d.box[1] = th; d.box[2] = std::max(1, std::min(T, TG_BM / (tw * th))); d.box[3] = 1;
-    d.ntaps = 27;
+    TapGemmParams p{};
+    p.on[0] = W; p.on[1] = H; p.on[2] = T; p.on[3] = 1;
+    conv_box(H, W, T, p.box);
+    p.ntaps = 27;
     for (int q = 0; q < 3; ++q)
         for (int r = 0; r < 3; ++r)
             for (int s = 0; s < 3; ++s) {
-                int* tp = d.tap[(q * 3 + r) * 3 + s];
+                int* tp = p.tap[(q * 3 + r) * 3 + s];
                 tp[0] = s - 1; tp[1] = r - 1; tp[2] = q;
             }
-    d.K = Cin; d.N = Cout;
-    d.W = W27; d.bias = bias; d.residual = residual; d.ldres = ldres;
-    d.out = out; d.ldo = ldo;
-    return launch_tapgemm(d, (cudaStream_t)stream);
+    p.K = Cin; p.N = Cout;
+    p.bias = (const __half*)bias; p.residual = (const __half*)residual; p.res_ld = ldres;
+    p.out = (__half*)out; p.out_ld = ldo;
+    return launch_tapgemm(p, X, Cin, W, H, T + 2, 1, W27, (cudaStream_t)stream);
 }
 
 long long star_conv2d_c4_workspace_bytes(int BT, int H, int W, int Cout) {

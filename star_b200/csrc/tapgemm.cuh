@@ -99,7 +99,7 @@ enum TapGemmEpi : int {
 };
 
 // The combinations the library's callers pass (UNet, OpenCLIP text tower, CogVideoX DiT, both VAEs), and the generic
-// instance.  Kinds with TG_EPI_GEGLU are compiled only at the tile widths GEGLU runs with (128 / 256).
+// instance.  Kinds with TG_EPI_GEGLU are compiled only at the tile widths GEGLU runs with (128 / 256): see tg_instance.
 #define TG_EPI_KINDS(X)                                   \
     X(0)                                                  \
     X(TG_EPI_BIAS)                                        \
@@ -111,6 +111,9 @@ enum TapGemmEpi : int {
     X(TG_EPI_BIAS | TG_EPI_TANH)                          \
     X(TG_EPI_BIAS | TG_EPI_COLSCALE | TG_EPI_RES)         \
     X(TG_EPI_GENERIC)
+
+// Whether instance <BN, EPI> of a kind in TG_EPI_KINDS is compiled: every one except the GEGLU kinds at BN = 160.
+constexpr bool tg_instance(int bn, int epi) { return !(bn == 160 && (epi & TG_EPI_GEGLU)); }
 
 // The kind of a call: its flags and which epilogue inputs it passes.
 inline int tg_epi_kind(int flags, bool bias, bool rowvec, bool colscale, bool residual) {

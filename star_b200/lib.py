@@ -90,23 +90,21 @@ def get_lib(dtype=None):
     return lib
 
 
-def last_error(dtype=None):
-    return get_lib(dtype).star_last_error().decode(errors="replace")
+def check(L, rc, what):
+    """Raises StarError with library L's message for the failed call ``what`` (rc != 0)."""
+    if rc != 0:
+        raise StarError(f"{what}: {L.star_last_error().decode(errors='replace')}")
 
 
 def ensure_init(device_index, dtype=None):
     key = (_key(dtype), device_index)
     if key in _inited:
         return
-    rc = get_lib(dtype).star_init(int(device_index))
-    if rc != 0:
-        raise StarError("star_init failed: " + last_error(dtype))
+    L = get_lib(dtype)
+    check(L, L.star_init(int(device_index)), "star_init failed")
     _inited.add(key)
 
 
-_last = [None]
-
-
-def check(rc, what):
-    if rc != 0:
-        raise StarError(f"{what}: {last_error(_last[0])}")
+def launch_count():
+    """Kernels launched by the loaded libraries since load (the fp16 one is loaded if none is)."""
+    return sum(L.star_launch_count() for L in _libs.values()) if _libs else get_lib().star_launch_count()

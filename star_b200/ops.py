@@ -65,33 +65,21 @@ def _traced(fn):
 
 def launch_count():
     """Kernels launched by the star_b200 libraries since load."""
-    return sum(lib.star_launch_count() for lib in _L._libs.values()) if _L._libs else _L.get_lib().star_launch_count()
+    return _L.launch_count()
 
 
-# Token dtype of the op in flight: fp16 (libstar_sm100.so) or bf16 (libstar_sm100_bf16.so, same sources).  Set by _dev() from
-# the op's first tensor (or its explicit ``dtype=``); every allocation and dtype check inside the op follows it.
-_cur = [torch.float16]
-
-
-def _dt():
-    return _cur[0]
-
-
-def _lib():
-    return _L.get_lib(_cur[0])
-
-
-def _dev(t, dtype=None):
+def _bind(t, dtype=None):
+    """(library, token dtype) of an op whose first tensor is t: fp16 tokens run on libstar_sm100.so, bf16 tokens on
+    libstar_sm100_bf16.so (same sources).  The dtype is t's (fp16 for other dtypes) or the explicit ``dtype=``; every
+    allocation and dtype check of the op follows it.  The library is initialised on t's device."""
     if not t.is_cuda:
         raise _L.StarError("star_b200 ops need CUDA tensors (no CPU fallback)")
     if dtype is None:
         dtype = t.dtype if t.dtype in (torch.float16, torch.bfloat16) else torch.float16
     if dtype not in (torch.float16, torch.bfloat16):
         raise _L.StarError(f"star_b200 ops run on fp16 or bf16 tokens, not {dtype}")
-    _cur[0] = dtype
-    _L._last[0] = dtype
     _L.ensure_init(t.device.index if t.device.index is not None else torch.cuda.current_device(), dtype)
-    return t.device
+    return _L.get_lib(dtype), dtype
 
 
 def _p(t):
@@ -102,9 +90,9 @@ def _st():
     return torch.cuda.current_stream().cuda_stream
 
 
-def _h(t, name):
-    if t is not None and t.dtype != _cur[0]:
-        raise _L.StarError(f"{name} must be {_cur[0]} like the op's first tensor, got {t.dtype}")
+def _h(t, name, dtype):
+    if t is not None and t.dtype != dtype:
+        raise _L.StarError(f"{name} must be {dtype} like the op's first tensor, got {t.dtype}")
     return t
 
 
@@ -118,55 +106,52 @@ def _rowmajor(t, name):
 @_traced
 def linear(a, w, bias=None, residual=None, rowvec=None, rowvec_div=1, flags=0, out=None):
     """out[r, n] = epi(sum_k a[r, k] w[n, k]); a may be a strided 2-D view."""
-    _dev(a)
-    _h(a, "a"); _h(w, "w"); _h(bias, "bias"); _h(residual, "residual"); _h(rowvec, "rowvec")
+    L, dt = _bind(a)
+    _h(a, "a", dt); _h(w, "w", dt); _h(bias, "bias", dt); _h(residual, "residual", dt); _h(rowvec, "rowvec", dt)
     lda = _rowmajor(a, "a")
     rows, K = a.shape
     n_w = w.shape[0]
     N = n_w // 2 if (flags & FLAG_GEGLU) else n_w
     assert w.is_contiguous() and w.shape[1] == K
     if out is None:
-        out = torch.empty((rows, N), dtype=_dt(), device=a.device)
+        out = torch.empty((rows, N), dtype=dt, device=a.device)
     ldo = _rowmajor(out, "out")
     ldres = _rowmajor(residual, "residual") if residual is not None else 0
     if rowvec is not None:
         assert rowvec.is_contiguous() and rowvec.shape[-1] == N
-    L = _lib()
-    _L.check(L.star_linear(_p(a), lda, _p(w), _p(bias), _p(rowvec), int(rowvec_div), _p(residual), ldres,
-                           _p(out), ldo, rows, K, N, flags, _st()), "star_linear")
+    _L.check(L, L.star_linear(_p(a), lda, _p(w), _p(bias), _p(rowvec), int(rowvec_div), _p(residual), ldres,
+                              _p(out), ldo, rows, K, N, flags, _st()), "star_linear")
     return out
 
 
 @_traced
 def conv2d_3x3(x, w9, bias=None, rowvec=None, rowvec_div=1, residual=None, out=None):
     """x [BT, H, W, Cin] contiguous; w9 [Cout, 3, 3, Cin]; returns [BT*H*W, Cout]."""
-    _dev(x)
+    L, dt = _bind(x)
     BT, H, W, Cin = x.shape
     Cout = w9.shape[0]
     assert x.is_contiguous() and w9.is_contiguous() and w9.shape[1:] == (3, 3, Cin)
     if out is None:
-        out = torch.empty((BT * H * W, Cout), dtype=_dt(), device=x.device)
+        out = torch.empty((BT * H * W, Cout), dtype=dt, device=x.device)
     ldo = _rowmajor(out, "out")
     ldres = _rowmajor(residual, "residual") if residual is not None else 0
     ldrv = _rowmajor(rowvec, "rowvec") if rowvec is not None else 0           # a column slice of a wider matrix is fine
-    L = _lib()
-    _L.check(L.star_conv2d_3x3(_p(x), _p(w9), _p(bias), _p(rowvec), int(rowvec_div), ldrv, _p(residual), ldres,
-                               _p(out), ldo, BT, H, W, Cin, Cout, _st()), "star_conv2d_3x3")
+    _L.check(L, L.star_conv2d_3x3(_p(x), _p(w9), _p(bias), _p(rowvec), int(rowvec_div), ldrv, _p(residual), ldres,
+                                  _p(out), ldo, BT, H, W, Cin, Cout, _st()), "star_conv2d_3x3")
     return out
 
 
 @_traced
 def conv2d_3x3_s2(x, w9, bias=None):
     """Downsample conv: stride 2, padding (2, 1).  x [BT,H,W,Cin] -> ([BT*Ho*Wo, Cout], Ho, Wo)."""
-    _dev(x)
+    L, dt = _bind(x)
     BT, H, W, Cin = x.shape
     Cout = w9.shape[0]
     assert x.is_contiguous() and w9.is_contiguous()
     Ho, Wo = (H + 1) // 2 + 1, (W - 1) // 2 + 1
-    L = _lib()
     ws = torch.empty(L.star_conv2d_s2_workspace_bytes(BT, H, W, Cin), dtype=torch.uint8, device=x.device)
-    out = torch.empty((BT * Ho * Wo, Cout), dtype=_dt(), device=x.device)
-    _L.check(L.star_conv2d_3x3_s2(_p(x), _p(w9), _p(bias), _p(out), Cout, _p(ws), BT, H, W, Cin, Cout, _st()),
+    out = torch.empty((BT * Ho * Wo, Cout), dtype=dt, device=x.device)
+    _L.check(L, L.star_conv2d_3x3_s2(_p(x), _p(w9), _p(bias), _p(out), Cout, _p(ws), BT, H, W, Cin, Cout, _st()),
              "star_conv2d_3x3_s2")
     return out, Ho, Wo
 
@@ -174,33 +159,31 @@ def conv2d_3x3_s2(x, w9, bias=None):
 @_traced
 def conv2d_3x3_s2p(x, w9, bias=None, pad=(0, 1, 0, 1)):
     """Stride-2 3x3 conv with explicit zero padding pad = (top, bottom, left, right).  Returns (out, Ho, Wo)."""
-    _dev(x)
+    L, dt = _bind(x)
     BT, H, W, Cin = x.shape
     Cout = w9.shape[0]
     assert x.is_contiguous() and w9.is_contiguous()
     pt, pb, pl, pr = (int(v) for v in pad)
     Ho, Wo = (H + pt + pb - 3) // 2 + 1, (W + pl + pr - 3) // 2 + 1
-    L = _lib()
     ws = torch.empty(L.star_conv2d_s2p_workspace_bytes(BT, H, W, Cin, pt, pb, pl, pr), dtype=torch.uint8, device=x.device)
-    out = torch.empty((BT * Ho * Wo, Cout), dtype=_dt(), device=x.device)
-    _L.check(L.star_conv2d_3x3_s2p(_p(x), _p(w9), _p(bias), _p(out), Cout, _p(ws), BT, H, W, Cin, Cout, pt, pb, pl, pr,
-                                   _st()), "star_conv2d_3x3_s2p")
+    out = torch.empty((BT * Ho * Wo, Cout), dtype=dt, device=x.device)
+    _L.check(L, L.star_conv2d_3x3_s2p(_p(x), _p(w9), _p(bias), _p(out), Cout, _p(ws), BT, H, W, Cin, Cout, pt, pb, pl, pr,
+                                      _st()), "star_conv2d_3x3_s2p")
     return out, Ho, Wo
 
 
 @_traced
 def conv_t3(x, w3, bias=None, residual=None, B=1, T=1, HW=1, out=None):
     """Temporal conv (3,1,1): x [B*T*HW, Cin]; w3 [Cout, 3, Cin]."""
-    _dev(x)
+    L, dt = _bind(x)
     rows, Cin = x.shape
     assert rows == B * T * HW and x.is_contiguous() and w3.is_contiguous()
     Cout = w3.shape[0]
     if out is None:
-        out = torch.empty((rows, Cout), dtype=_dt(), device=x.device)
+        out = torch.empty((rows, Cout), dtype=dt, device=x.device)
     ldres = _rowmajor(residual, "residual") if residual is not None else 0
-    L = _lib()
-    _L.check(L.star_conv_t3(_p(x), _p(w3), _p(bias), _p(residual), ldres, _p(out), _rowmajor(out, "out"),
-                            B, T, HW, Cin, Cout, _st()), "star_conv_t3")
+    _L.check(L, L.star_conv_t3(_p(x), _p(w3), _p(bias), _p(residual), ldres, _p(out), _rowmajor(out, "out"),
+                               B, T, HW, Cin, Cout, _st()), "star_conv_t3")
     return out
 
 
@@ -208,17 +191,16 @@ def conv_t3(x, w3, bias=None, residual=None, B=1, T=1, HW=1, out=None):
 def conv3d_causal(xp, w27, T, H, W, bias=None, residual=None, out=None):
     """Causal Conv3d 3x3x3 (CogVideoX VAE).  xp [(T+2)*H*W, Cin]: two context frames + the clip; w27 [Cout, 3, 3, 3, Cin];
     returns [T*H*W, Cout]."""
-    _dev(xp)
+    L, dt = _bind(xp)
     rows, Cin = xp.shape
     assert rows == (T + 2) * H * W and xp.is_contiguous() and w27.is_contiguous() and tuple(w27.shape[1:]) == (3, 3, 3, Cin)
-    _h(w27, "w27"); _h(bias, "bias"); _h(residual, "residual")
+    _h(w27, "w27", dt); _h(bias, "bias", dt); _h(residual, "residual", dt)
     Cout = w27.shape[0]
     if out is None:
-        out = torch.empty((T * H * W, Cout), dtype=_dt(), device=xp.device)
+        out = torch.empty((T * H * W, Cout), dtype=dt, device=xp.device)
     ldres = _rowmajor(residual, "residual") if residual is not None else 0
-    L = _lib()
-    _L.check(L.star_conv3d_causal(_p(xp), _p(w27), _p(bias), _p(residual), ldres, _p(out), _rowmajor(out, "out"),
-                                  T, H, W, Cin, Cout, _st()), "star_conv3d_causal")
+    _L.check(L, L.star_conv3d_causal(_p(xp), _p(w27), _p(bias), _p(residual), ldres, _p(out), _rowmajor(out, "out"),
+                                     T, H, W, Cin, Cout, _st()), "star_conv3d_causal")
     return out
 
 
@@ -226,34 +208,32 @@ def conv3d_causal(xp, w27, T, H, W, bias=None, residual=None, out=None):
 def groupnorm_mod(x, gamma, beta, ymod, bmod, T, H, W, Tl, Hl, Wl, eps, silu, out=None):
     """SpatialNorm3D: GroupNorm32 over one clip x [T*H*W, C], times ymod[src] plus bmod[src] (latent-resolution
     [Tl*Hl*Wl, C] tables, nearest-neighbour gather with the reference's first-frame split), optional SiLU."""
-    _dev(x)
+    L, dt = _bind(x)
     rows, C = x.shape
     assert rows == T * H * W and x.is_contiguous()
     assert tuple(ymod.shape) == (Tl * Hl * Wl, C) and tuple(bmod.shape) == (Tl * Hl * Wl, C)
     ldmod = _rowmajor(ymod, "ymod")                      # column slices of one [rows, 2C] GEMM result are fine
     assert _rowmajor(bmod, "bmod") == ldmod
-    _h(gamma, "gamma"); _h(beta, "beta"); _h(ymod, "ymod"); _h(bmod, "bmod")
-    L = _lib()
+    _h(gamma, "gamma", dt); _h(beta, "beta", dt); _h(ymod, "ymod", dt); _h(bmod, "bmod", dt)
     ws = torch.empty(L.star_groupnorm_workspace_bytes(1, C), dtype=torch.uint8, device=x.device)
     if out is None:
         out = torch.empty_like(x)
     assert out.is_contiguous() and out.shape == x.shape and out.dtype == x.dtype
-    _L.check(L.star_groupnorm_mod(_p(x), _p(gamma), _p(beta), _p(ymod), _p(bmod), ldmod, _p(out), T, H, W, Tl, Hl, Wl, C,
-                                  float(eps), int(bool(silu)), _p(ws), _st()), "star_groupnorm_mod")
+    _L.check(L, L.star_groupnorm_mod(_p(x), _p(gamma), _p(beta), _p(ymod), _p(bmod), ldmod, _p(out), T, H, W, Tl, Hl, Wl, C,
+                                     float(eps), int(bool(silu)), _p(ws), _st()), "star_groupnorm_mod")
     return out
 
 
 @_traced
 def conv2d_3x3_c4(x, w9, bias=None, residual=None):
     """Stem conv, x [BT, H, W, 4]; w9 [Cout, 3, 3, 4]."""
-    _dev(x)
+    L, dt = _bind(x)
     BT, H, W, C = x.shape
     assert C == 4 and x.is_contiguous() and w9.is_contiguous()
     Cout = w9.shape[0]
-    out = torch.empty((BT * H * W, Cout), dtype=_dt(), device=x.device)
-    L = _lib()
+    out = torch.empty((BT * H * W, Cout), dtype=dt, device=x.device)
     ws = torch.empty(L.star_conv2d_c4_workspace_bytes(BT, H, W, Cout), dtype=torch.uint8, device=x.device)
-    _L.check(L.star_conv2d_3x3_c4(_p(x), _p(w9), _p(bias), _p(residual), _p(out), _p(ws), BT, H, W, Cout, _st()),
+    _L.check(L, L.star_conv2d_3x3_c4(_p(x), _p(w9), _p(bias), _p(residual), _p(out), _p(ws), BT, H, W, Cout, _st()),
              "star_conv2d_3x3_c4")
     return out
 
@@ -261,36 +241,33 @@ def conv2d_3x3_c4(x, w9, bias=None, residual=None):
 @_traced
 def attention(q, k, v, batch, heads, Nq, Nk, kv_batch_div=1, scale=0.125, out=None):
     """q [batch*Nq, >=heads*64] / k, v [kv_batches*Nk, ...] strided 2-D views (head h at columns h*64..)."""
-    _dev(q)
+    L, dt = _bind(q)
     ldq, ldk, ldv = _rowmajor(q, "q"), _rowmajor(k, "k"), _rowmajor(v, "v")
     if out is None:
-        out = torch.empty((batch * Nq, heads * 64), dtype=_dt(), device=q.device)
-    L = _lib()
-    _L.check(L.star_attention(_p(q), ldq, _p(k), ldk, _p(v), ldv, _p(out), _rowmajor(out, "out"), batch, heads,
-                              Nq, Nk, kv_batch_div, float(scale), _st()), "star_attention")
+        out = torch.empty((batch * Nq, heads * 64), dtype=dt, device=q.device)
+    _L.check(L, L.star_attention(_p(q), ldq, _p(k), ldk, _p(v), ldv, _p(out), _rowmajor(out, "out"), batch, heads,
+                                 Nq, Nk, kv_batch_div, float(scale), _st()), "star_attention")
     return out
 
 
 @_traced
 def attention_causal(q, k, v, batch, heads, N, scale=0.125, out=None):
     """causal self-attention (query i sees keys 0..i): q, k, v [batch*N, >=heads*64] strided 2-D views"""
-    _dev(q)
+    L, dt = _bind(q)
     ldq, ldk, ldv = _rowmajor(q, "q"), _rowmajor(k, "k"), _rowmajor(v, "v")
     if out is None:
-        out = torch.empty((batch * N, heads * 64), dtype=_dt(), device=q.device)
-    L = _lib()
-    _L.check(L.star_attention_causal(_p(q), ldq, _p(k), ldk, _p(v), ldv, _p(out), _rowmajor(out, "out"), batch, heads, N,
-                                     float(scale), _st()), "star_attention_causal")
+        out = torch.empty((batch * N, heads * 64), dtype=dt, device=q.device)
+    _L.check(L, L.star_attention_causal(_p(q), ldq, _p(k), ldk, _p(v), ldv, _p(out), _rowmajor(out, "out"), batch, heads, N,
+                                        float(scale), _st()), "star_attention_causal")
     return out
 
 
 @_traced
 def temporal_attention(qkv, B, T, HW, heads, Ci, scale=0.125):
-    _dev(qkv)
+    L, dt = _bind(qkv)
     ld = _rowmajor(qkv, "qkv")
-    out = torch.empty((qkv.shape[0], Ci), dtype=_dt(), device=qkv.device)
-    L = _lib()
-    _L.check(L.star_temporal_attention(_p(qkv), ld, _p(out), Ci, B, T, HW, heads, Ci, float(scale), _st()),
+    out = torch.empty((qkv.shape[0], Ci), dtype=dt, device=qkv.device)
+    _L.check(L, L.star_temporal_attention(_p(qkv), ld, _p(out), Ci, B, T, HW, heads, Ci, float(scale), _st()),
              "star_temporal_attention")
     return out
 
@@ -298,122 +275,112 @@ def temporal_attention(qkv, B, T, HW, heads, Ci, scale=0.125):
 @_traced
 def groupnorm(x, gamma, beta, nsamples, eps, silu, out=None):
     """x [rows, C]; nsamples equal blocks of rows share statistics.  out may alias x (in place)."""
-    _dev(x)
+    L, _ = _bind(x)
     rows, C = x.shape
     assert x.is_contiguous() and rows % nsamples == 0
-    L = _lib()
     ws = torch.empty(L.star_groupnorm_workspace_bytes(nsamples, C), dtype=torch.uint8, device=x.device)
     if out is None:
         out = torch.empty_like(x)
     assert out.is_contiguous() and out.shape == x.shape
-    _L.check(L.star_groupnorm(_p(x), _p(gamma), _p(beta), _p(out), nsamples, rows // nsamples, C, float(eps),
-                              int(bool(silu)), _p(ws), _st()), "star_groupnorm")
+    _L.check(L, L.star_groupnorm(_p(x), _p(gamma), _p(beta), _p(out), nsamples, rows // nsamples, C, float(eps),
+                                 int(bool(silu)), _p(ws), _st()), "star_groupnorm")
     return out
 
 
 @_traced
 def layernorm(x, gamma, beta, gate_mode=0, gate=None, w0=0.0, w1=0.0, eps=1e-5):
-    _dev(x)
+    L, _ = _bind(x)
     rows, C = x.shape
     assert x.is_contiguous()
     out = torch.empty_like(x)
-    L = _lib()
-    _L.check(L.star_layernorm(_p(x), _p(gamma), _p(beta), _p(out), rows, C, float(eps), gate_mode, _p(gate),
-                              float(w0), float(w1), _st()), "star_layernorm")
+    _L.check(L, L.star_layernorm(_p(x), _p(gamma), _p(beta), _p(out), rows, C, float(eps), gate_mode, _p(gate),
+                                 float(w0), float(w1), _st()), "star_layernorm")
     return out
 
 
 @_traced
 def liem_spatial_gate(x, w98, BT, H, W):
-    _dev(x)
+    L, dt = _bind(x)
     rows, C = x.shape
     assert rows == BT * H * W and x.is_contiguous()
-    mm = torch.empty((rows, 2), dtype=_dt(), device=x.device)
-    gate = torch.empty((rows,), dtype=_dt(), device=x.device)
-    L = _lib()
-    _L.check(L.star_liem_spatial_gate(_p(x), _p(w98), _p(mm), _p(gate), BT, H, W, C, _st()),
+    mm = torch.empty((rows, 2), dtype=dt, device=x.device)
+    gate = torch.empty((rows,), dtype=dt, device=x.device)
+    _L.check(L, L.star_liem_spatial_gate(_p(x), _p(w98), _p(mm), _p(gate), BT, H, W, C, _st()),
              "star_liem_spatial_gate")
     return gate
 
 
 @_traced
 def concat_add(a, b, c=None):
-    _dev(a)
+    L, dt = _bind(a)
     rows, Ca = a.shape
     Cb = b.shape[1]
     assert a.is_contiguous() and b.is_contiguous() and (c is None or c.is_contiguous())
-    out = torch.empty((rows, Ca + Cb), dtype=_dt(), device=a.device)
-    L = _lib()
-    _L.check(L.star_concat_add(_p(a), Ca, _p(b), _p(c), Cb, _p(out), rows, _st()), "star_concat_add")
+    out = torch.empty((rows, Ca + Cb), dtype=dt, device=a.device)
+    _L.check(L, L.star_concat_add(_p(a), Ca, _p(b), _p(c), Cb, _p(out), rows, _st()), "star_concat_add")
     return out
 
 
 @_traced
 def add(a, b):
-    _dev(a)
+    L, _ = _bind(a)
     assert a.is_contiguous() and b.is_contiguous() and a.shape == b.shape
     out = torch.empty_like(a)
-    L = _lib()
-    _L.check(L.star_add(_p(a), _p(b), _p(out), a.numel(), _st()), "star_add")
+    _L.check(L, L.star_add(_p(a), _p(b), _p(out), a.numel(), _st()), "star_add")
     return out
 
 
 @_traced
 def time_avgpool2(x, T, HW):
     """frame-pair average of a [(T HW), C] clip (odd T: first frame kept): -> [(ceil(T/2) HW), C]"""
-    _dev(x)
+    L, dt = _bind(x)
     C = x.shape[1]
     assert x.is_contiguous() and x.shape[0] == T * HW
     To = (T + 1) // 2 if T % 2 else T // 2
-    out = torch.empty((To * HW, C), dtype=_dt(), device=x.device)
-    L = _lib()
-    _L.check(L.star_time_avgpool2(_p(x), _p(out), T, HW, C, _st()), "star_time_avgpool2")
+    out = torch.empty((To * HW, C), dtype=dt, device=x.device)
+    _L.check(L, L.star_time_avgpool2(_p(x), _p(out), T, HW, C, _st()), "star_time_avgpool2")
     return out
 
 
 @_traced
 def upsample2x_crop(x, BT, H, W):
-    _dev(x)
+    L, dt = _bind(x)
     C = x.shape[1]
-    out = torch.empty((BT * (2 * H - 2) * (2 * W), C), dtype=_dt(), device=x.device)
-    L = _lib()
-    _L.check(L.star_upsample2x_crop(_p(x), _p(out), BT, H, W, C, _st()), "star_upsample2x_crop")
+    out = torch.empty((BT * (2 * H - 2) * (2 * W), C), dtype=dt, device=x.device)
+    _L.check(L, L.star_upsample2x_crop(_p(x), _p(out), BT, H, W, C, _st()), "star_upsample2x_crop")
     return out
 
 
 @_traced
 def upsample2x(x, BT, H, W, out=None):
     """plain nearest x2: [BT*H*W, C] -> [BT*2H*2W, C]"""
-    _dev(x)
+    L, dt = _bind(x)
     C = x.shape[1]
     assert x.is_contiguous()
     if out is None:
-        out = torch.empty((BT * 4 * H * W, C), dtype=_dt(), device=x.device)
+        out = torch.empty((BT * 4 * H * W, C), dtype=dt, device=x.device)
     assert out.is_contiguous() and tuple(out.shape) == (BT * 4 * H * W, C)
-    L = _lib()
-    _L.check(L.star_upsample2x(_p(x), _p(out), BT, H, W, C, 0, _st()), "star_upsample2x")
+    _L.check(L, L.star_upsample2x(_p(x), _p(out), BT, H, W, C, 0, _st()), "star_upsample2x")
     return out
 
 
 @_traced
 def softmax_rows(s, cols):
     """in-place row softmax of the fp16 matrix s[rows, ld] over its first `cols` columns"""
-    _dev(s)
+    L, _ = _bind(s)
     ld = _rowmajor(s, "s")
-    L = _lib()
-    _L.check(L.star_softmax_rows(_p(s), ld, s.shape[0], int(cols), _st()), "star_softmax_rows")
+    _L.check(L, L.star_softmax_rows(_p(s), ld, s.shape[0], int(cols), _st()), "star_softmax_rows")
     return s
 
 
 @_traced
 def vae_head(x, w27, bias3, B, T, H, W):
     """x [(b t h w), ld>=3] -> (B*T, 3, H, W) fp16 after the (3,1,1) temporal conv over t"""
-    _dev(x)
+    L, dt = _bind(x)
     ld = _rowmajor(x, "x")
     assert w27.is_contiguous() and w27.numel() == 27 and bias3.numel() == 3
-    out = torch.empty((B * T, 3, H, W), dtype=_dt(), device=x.device)
-    L = _lib()
-    _L.check(L.star_vae_head(_p(x), ld, _p(_h(w27, "w27")), _p(_h(bias3, "bias3")), _p(out), B, T, H * W, _st()),
+    out = torch.empty((B * T, 3, H, W), dtype=dt, device=x.device)
+    _L.check(L, L.star_vae_head(_p(x), ld, _p(_h(w27, "w27", dt)), _p(_h(bias3, "bias3", dt)), _p(out), B, T, H * W, _st()),
              "star_vae_head")
     return out
 
@@ -421,48 +388,44 @@ def vae_head(x, w27, bias3, B, T, H, W):
 @_traced
 def nchw5_to_tokens(x, dtype=torch.float16):
     """(b, c, f, h, w) fp32 -> [(b f h w), c] fp16 (or bf16)"""
-    _dev(x, dtype)
+    L, dt = _bind(x, dtype)
     x = x.contiguous().float()
     B, C, F, H, W = x.shape
-    out = torch.empty((B * F * H * W, C), dtype=_dt(), device=x.device)
-    L = _lib()
-    _L.check(L.star_nchw5_to_tokens(_p(x), _p(out), B, C, F, H * W, _st()), "star_nchw5_to_tokens")
+    out = torch.empty((B * F * H * W, C), dtype=dt, device=x.device)
+    _L.check(L, L.star_nchw5_to_tokens(_p(x), _p(out), B, C, F, H * W, _st()), "star_nchw5_to_tokens")
     return out
 
 
 @_traced
 def tokens_to_nchw5(x, B, C, F, H, W):
-    _dev(x)
-    out = torch.empty((B, C, F, H, W), dtype=_dt(), device=x.device)
-    L = _lib()
-    _L.check(L.star_tokens_to_nchw5(_p(x), _rowmajor(x, "x"), _p(out), B, C, F, H * W, _st()), "star_tokens_to_nchw5")
+    L, dt = _bind(x)
+    out = torch.empty((B, C, F, H, W), dtype=dt, device=x.device)
+    _L.check(L, L.star_tokens_to_nchw5(_p(x), _rowmajor(x, "x"), _p(out), B, C, F, H * W, _st()), "star_tokens_to_nchw5")
     return out
 
 
 @_traced
 def sinusoidal(t, dim, dtype=torch.float16):
-    _dev(t, dtype)
+    L, dt = _bind(t, dtype)
     t = t.to(torch.int64).contiguous()
-    out = torch.empty((t.shape[0], dim), dtype=_dt(), device=t.device)
-    L = _lib()
-    _L.check(L.star_sinusoidal(_p(t), _p(out), t.shape[0], dim, _st()), "star_sinusoidal")
+    out = torch.empty((t.shape[0], dim), dtype=dt, device=t.device)
+    _L.check(L, L.star_sinusoidal(_p(t), _p(out), t.shape[0], dim, _st()), "star_sinusoidal")
     return out
 
 
 @_traced
 def silu(x):
-    _dev(x)
+    L, _ = _bind(x)
     assert x.is_contiguous()
     out = torch.empty_like(x)
-    L = _lib()
-    _L.check(L.star_silu(_p(x), _p(out), x.numel(), _st()), "star_silu")
+    _L.check(L, L.star_silu(_p(x), _p(out), x.numel(), _st()), "star_silu")
     return out
 
 
 @_traced
 def bilinear_pad(x, H, W, padding=(0, 0, 0, 0), value=1.0):
     """F.interpolate(x, [H, W], mode='bilinear') + F.pad(x, padding=(l, r, t, b), 'constant', value); x fp32 (..., h, w)"""
-    _dev(x)
+    L, _ = _bind(x)
     if x.dtype != torch.float32:
         raise _L.StarError("bilinear_pad expects fp32 frames")
     x = x.contiguous()
@@ -472,8 +435,7 @@ def bilinear_pad(x, H, W, padding=(0, 0, 0, 0), value=1.0):
     nc = 1
     for d in lead:
         nc *= d
-    L = _lib()
-    _L.check(L.star_bilinear_pad(_p(x), _p(out), nc, h, w, int(H), int(W), pl, pr, pt, pb, float(value), _st()),
+    _L.check(L, L.star_bilinear_pad(_p(x), _p(out), nc, h, w, int(H), int(W), pl, pr, pt, pb, float(value), _st()),
              "star_bilinear_pad")
     return out
 
@@ -482,16 +444,15 @@ def bilinear_pad(x, H, W, padding=(0, 0, 0, 0), value=1.0):
 def adain_color_fix(video, source, uint8=False):
     """tensor2vid + adain_color_fix on the GPU: video (1, C, F, H, W) fp32 in [-1, 1] (test()'s result), source (F, C, h, w) fp32 in
     [-1, 1] (the LR clip) -> (F, H, W, C) in [0, 255], fp32 like the reference or uint8 (rounded; 4x less D2H traffic)."""
-    _dev(video)
+    L, _ = _bind(video)
     assert video.dim() == 5 and video.shape[0] == 1 and video.dtype == torch.float32 and source.dtype == torch.float32
     _, C, F, H, W = video.shape
     assert source.shape[0] == F and source.shape[1] == C
     video, source = video.contiguous(), source.to(video.device).contiguous()
     out = torch.empty((F, H, W, C), dtype=torch.uint8 if uint8 else torch.float32, device=video.device)
-    L = _lib()
     ws = torch.empty(L.star_adain_workspace_bytes(C, F), dtype=torch.uint8, device=video.device)
-    _L.check(L.star_adain_color_fix(_p(video), _p(source), None if uint8 else _p(out), _p(out) if uint8 else None, C, F, H * W,
-                                    source.shape[2] * source.shape[3], _p(ws), _st()), "star_adain_color_fix")
+    _L.check(L, L.star_adain_color_fix(_p(video), _p(source), None if uint8 else _p(out), _p(out) if uint8 else None, C, F, H * W,
+                                       source.shape[2] * source.shape[3], _p(ws), _st()), "star_adain_color_fix")
     return out
 
 
@@ -517,10 +478,10 @@ def cfg_x0(y_out, u_out, xt, alphas, sigmas, guide_scale, guide_rescale=None, re
     (B, C, F, H, W) fp32 contiguous, read in place at the tile's window, and x0 is not returned but accumulated:
     blend.acc[:, :, f0 + lo:f0 + hi, r0:r0 + th, c0:c0 + tw] += wy[:, None] * wx[None, :] * x0[:, :, lo:hi]; returns blend.acc.
     The rescale statistics span the whole tile output."""
-    _dev(y_out)
-    _h(y_out, "y_out"); _h(u_out, "u_out")
+    L, dt = _bind(y_out)
+    _h(y_out, "y_out", dt); _h(u_out, "u_out", dt)
     if blend is not None:
-        return _cfg_x0_blend(y_out, u_out, xt, alphas, sigmas, guide_scale, guide_rescale, return_guided, blend)
+        return _cfg_x0_blend(L, y_out, u_out, xt, alphas, sigmas, guide_scale, guide_rescale, return_guided, blend)
     assert y_out.is_contiguous() and u_out.is_contiguous() and y_out.shape == u_out.shape == xt.shape
     B = y_out.shape[0]
     per = y_out.numel() // B
@@ -529,15 +490,14 @@ def cfg_x0(y_out, u_out, xt, alphas, sigmas, guide_scale, guide_rescale=None, re
     guided = torch.empty_like(y_out) if return_guided else None
     al = alphas.reshape(B).float().contiguous()
     sg = sigmas.reshape(B).float().contiguous()
-    L = _lib()
     ws = torch.empty(L.star_cfg_x0_workspace_bytes(B), dtype=torch.uint8, device=y_out.device)
-    _L.check(L.star_cfg_x0(_p(y_out), _p(u_out), _p(xt), _p(x0), _p(guided), float(guide_scale),
-                           -1.0 if guide_rescale is None else float(guide_rescale), _p(al), _p(sg), B, per, _p(ws), _st()),
+    _L.check(L, L.star_cfg_x0(_p(y_out), _p(u_out), _p(xt), _p(x0), _p(guided), float(guide_scale),
+                              -1.0 if guide_rescale is None else float(guide_rescale), _p(al), _p(sg), B, per, _p(ws), _st()),
              "star_cfg_x0")
     return (x0, guided) if return_guided else x0
 
 
-def _cfg_x0_blend(y_out, u_out, xt, alphas, sigmas, guide_scale, guide_rescale, return_guided, blend):
+def _cfg_x0_blend(L, y_out, u_out, xt, alphas, sigmas, guide_scale, guide_rescale, return_guided, blend):
     if return_guided:
         raise ValueError("cfg_x0: return_guided is not available with blend=")
     acc = blend.acc
@@ -556,12 +516,11 @@ def _cfg_x0_blend(y_out, u_out, xt, alphas, sigmas, guide_scale, guide_rescale, 
     _, _, F, H, W = xt.shape
     al = alphas.reshape(B).float().contiguous()
     sg = sigmas.reshape(B).float().contiguous()
-    L = _lib()
     ws = torch.empty(L.star_cfg_x0_workspace_bytes(B), dtype=torch.uint8, device=y_out.device)
-    _L.check(L.star_cfg_x0_blend(_p(y_out), _p(u_out), _p(xt), _p(acc), float(guide_scale),
-                                 -1.0 if guide_rescale is None else float(guide_rescale), _p(al), _p(sg), _p(blend.wy),
-                                 _p(blend.wx), B, C, Ft, th, tw, F, H, W, int(blend.f0), int(blend.lo), int(blend.hi),
-                                 int(blend.r0), int(blend.c0), _p(ws), _st()),
+    _L.check(L, L.star_cfg_x0_blend(_p(y_out), _p(u_out), _p(xt), _p(acc), float(guide_scale),
+                                    -1.0 if guide_rescale is None else float(guide_rescale), _p(al), _p(sg), _p(blend.wy),
+                                    _p(blend.wx), B, C, Ft, th, tw, F, H, W, int(blend.f0), int(blend.lo), int(blend.hi),
+                                    int(blend.r0), int(blend.c0), _p(ws), _st()),
              "star_cfg_x0_blend")
     return acc
 
@@ -572,39 +531,36 @@ FLAG_GELU_TANH = 8
 @_traced
 def linear_ex(a, w, bias=None, colscale=None, residual=None, flags=0, out=None):
     """out = residual + colscale[n] * act(sum_k a[r,k] w[n,k] + bias[n])   (adaLN-gated residual, tanh-GELU option)"""
-    _dev(a)
+    L, dt = _bind(a)
     lda = _rowmajor(a, "a")
     rows, K = a.shape
     N = w.shape[0]
     assert w.is_contiguous() and w.shape[1] == K
     if out is None:
-        out = torch.empty((rows, N), dtype=_dt(), device=a.device)
+        out = torch.empty((rows, N), dtype=dt, device=a.device)
     ldres = _rowmajor(residual, "residual") if residual is not None else 0
-    L = _lib()
-    _L.check(L.star_linear_ex(_p(a), lda, _p(w), _p(bias), None, 1, _p(colscale), _p(residual), ldres, _p(out),
-                              _rowmajor(out, "out"), rows, K, N, flags, _st()), "star_linear_ex")
+    _L.check(L, L.star_linear_ex(_p(a), lda, _p(w), _p(bias), None, 1, _p(colscale), _p(residual), ldres, _p(out),
+                                 _rowmajor(out, "out"), rows, K, N, flags, _st()), "star_linear_ex")
     return out
 
 
 @_traced
 def row_gate(x, mode, gate=None, w0=0.0, w1=0.0, out=None):
-    _dev(x)
+    L, _ = _bind(x)
     rows, C = x.shape
     assert x.is_contiguous()
     if out is None:
         out = torch.empty_like(x)
-    L = _lib()
-    _L.check(L.star_row_gate(_p(x), _p(out), rows, C, mode, _p(gate), float(w0), float(w1), _st()), "star_row_gate")
+    _L.check(L, L.star_row_gate(_p(x), _p(out), rows, C, mode, _p(gate), float(w0), float(w1), _st()), "star_row_gate")
     return out
 
 
 @_traced
 def qk_ln_rope(qkv, heads, koff, qg, qb, kg, kb, cos, sin, seq, text_len, eps=1e-6):
     """in place on qkv [rows, ld]"""
-    _dev(qkv)
+    L, _ = _bind(qkv)
     ld = _rowmajor(qkv, "qkv")
     assert cos.dtype == torch.float32 and sin.dtype == torch.float32 and cos.is_contiguous() and sin.is_contiguous()
-    L = _lib()
-    _L.check(L.star_qk_ln_rope(_p(qkv), ld, qkv.shape[0], heads, koff, _p(qg), _p(qb), _p(kg), _p(kb), _p(cos), _p(sin),
-                               seq, text_len, float(eps), _st()), "star_qk_ln_rope")
+    _L.check(L, L.star_qk_ln_rope(_p(qkv), ld, qkv.shape[0], heads, koff, _p(qg), _p(qb), _p(kg), _p(kb), _p(cos), _p(sin),
+                                  seq, text_len, float(eps), _st()), "star_qk_ln_rope")
     return qkv

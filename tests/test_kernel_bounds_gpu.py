@@ -11,10 +11,10 @@ linear op is proportional to M, the same fp64 reference evaluated on absolute va
 constants are derived in the block below, one reason each; none is fitted to observed errors.
 
 tests/util.py::assert_close bounds rel-L2 and max|err| / max|ref| and lets a wrong bias on one column, a single element a few
-ulps off or one mis-masked attention key pass; test_checker_catches_injected_faults shows which.  The case tables restate the
-host-side dispatch rules of star_abi.cu (tile width, box shape, temporal template) and test_case_tables_cover_every_path
-checks, on the CPU, that every tile width x {full, partial last column tile} x {plain, GEGLU}, every K-tail entry point and
-every temporal-attention template has a case.  Failures name the violating (row, col) positions, their tile and the worst
+ulps off or one mis-masked attention key pass; test_checker_catches_injected_faults shows which.  The case tables follow the
+host-side dispatch rules of star_abi.cu (tile width and box shape as tools/gemm_roofline.py restates them, temporal template)
+and test_case_tables_cover_every_path checks, on the CPU, that every tile width x {full, partial last column tile} x {plain,
+GEGLU}, every K-tail entry point and every temporal-attention template has a case.  Failures name the violating (row, col) positions, their tile and the worst
 error / bound ratio; passing cases print their worst ratio (pytest -s).
 """
 import math
@@ -25,6 +25,7 @@ import torch
 import torch.nn.functional as F
 
 from tests.util import assert_close
+from tools.gemm_roofline import geometry, tile_width
 
 HALF, BF16, F64 = torch.float16, torch.bfloat16, torch.float64
 
@@ -186,60 +187,17 @@ def attention_ref(q, k, v, batch, heads, nq, nk, div, scale, dtype, causal=False
     return back(y), back(b)
 
 
-# ---- tap-GEMM dispatch, restated from star_abi.cu ------------------------------------------------------------------------
+# ---- tap-GEMM dispatch (tile width and geometry: tools/gemm_roofline.py) ---------------------------------------------------
 def stages(bn):
     """TapGemmSmem<BN>::STAGES: (A 128x64 + W BNx64) fp16 stages in 227 KB, at most 8"""
     return min((232448 - 1024 - 256) // (128 * 64 * 2 + bn * 64 * 2), 8)
-
-
-def tile_width(n, geglu):
-    """launch_tapgemm: the tile width that pads N least, the wider on a tie (GEGLU: 64 or 128 value columns)"""
-    pad = lambda w: _ceil(n, w) * w                                              # noqa: E731
-    if geglu:
-        return 256 if pad(128) <= pad(64) else 128
-    if pad(256) <= pad(128) and pad(256) <= pad(160):
-        return 256
-    return 160 if pad(160) <= pad(128) else 128
-
-
-def best_box_2d(h, w):
-    best, th, tw = -1, 1, 1
-    for bw in range(1, min(w, 128) + 1):
-        bh = min(h, 128 // bw)
-        if bh < 1:
-            continue
-        t = _ceil(w, bw) * _ceil(h, bh)
-        if best < 0 or t < best or (t == best and bw > tw):
-            best, th, tw = t, bh, bw
-    return th, tw
-
-
-def tap_geometry(op, d):
-    """(output extents on[4], box[4], taps, K, N) of one entry point, as its TapDesc"""
-    if op in ("linear", "linear_ex"):
-        return (d["rows"], 1, 1, 1), (128, 1, 1, 1), 1, d["K"], d["N"]
-    if op == "conv2d_3x3":
-        th, tw = best_box_2d(d["H"], d["W"])
-        return (d["W"], d["H"], d["BT"], 1), (tw, th, max(1, min(d["BT"], 128 // (tw * th))), 1), 9, d["Cin"], d["Cout"]
-    if op == "conv2d_3x3_s2p":
-        pt, pb, pl, pr = d["pad"]
-        ho, wo = (d["H"] + pt + pb - 3) // 2 + 1, (d["W"] + pl + pr - 3) // 2 + 1
-        th, tw = best_box_2d(ho, wo)
-        return (wo, ho, 1, d["BT"]), (tw, th, 1, 1), 9, d["Cin"], d["Cout"]
-    if op == "conv_t3":
-        hw, t = d["HW"], d["T"]
-        return (hw, t, d["B"], 1), (min(128, hw), min(t, 128 // hw) if hw < 128 else 1, 1, 1), 3, d["Cin"], d["Cout"]
-    if op == "conv3d_causal":
-        th, tw = best_box_2d(d["H"], d["W"])
-        return (d["W"], d["H"], d["T"], 1), (tw, th, max(1, min(d["T"], 128 // (tw * th))), 1), 27, d["Cin"], d["Cout"]
-    raise ValueError(op)
 
 
 Plan = namedtuple("Plan", "bn npt n_tiles m_tiles tiles iters stages k16 on box")
 
 
 def plan(case):
-    on, box, taps, K, N = tap_geometry(case.op, case.d)
+    on, box, taps, K, N, _ = geometry(case.op, case.d)
     geglu = bool(case.flags & 1)
     bn = tile_width(N, geglu)
     npt = bn // 2 if geglu else bn
@@ -386,7 +344,7 @@ def run_gemm_case(O, case):
     """launch one case; returns (got, fp64 value, bound, locator, untouched-region check or None)"""
     d, op, dt, ex = case.d, case.op, case.dtype, case.extras
     pl = plan(case)
-    on, box, taps, K, N = tap_geometry(op, d)
+    on, box, taps, K, N, _ = geometry(op, d)
     geglu = bool(case.flags & 1)
     wrows = 2 * N if geglu else N
     if op in ("linear", "linear_ex"):
@@ -528,12 +486,12 @@ def test_case_tables_cover_every_path():
         pl = plan(case)
         assert pl.bn == case.bn, f"{case.id}: the tile-width rule picks {pl.bn}, the case expects {case.bn}"
         geglu = bool(case.flags & 1)
-        N = tap_geometry(case.op, case.d)[4]
+        N = geometry(case.op, case.d)[4]
         cells.add(("geglu" if geglu else "plain", pl.bn, "partial" if N % pl.npt else "full"))
         if pl.tiles > NUM_SMS:
             cells.add(("multi-tile", pl.bn))
         cells.add(("ring", pl.bn, "fewer" if pl.iters < pl.stages else "more"))
-        K = tap_geometry(case.op, case.d)[3]
+        K = geometry(case.op, case.d)[3]
         if K % 64:
             cells.add(("ktail", case.op.replace("linear_ex", "linear"), K))
         if case.op in ("conv2d_3x3", "conv3d_causal"):

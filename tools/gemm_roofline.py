@@ -33,7 +33,7 @@ def _ceil(a, b):
     return -(-a // b)
 
 
-# ---- dispatch, restated from star_abi.cu -----------------------------------------------------------------------------------
+# ---- dispatch, restated from star_abi.cu (the one Python copy: tests/test_kernel_bounds_gpu.py plans its cases with it) ----
 def tile_width(n, geglu):
     """launch_tapgemm: the tile width that pads N least, the wider on a tie (GEGLU: 64 or 128 value columns)"""
     pad = lambda w: _ceil(n, w) * w                                              # noqa: E731
@@ -64,6 +64,7 @@ def epi_instance(flags, epi):
 
 
 def best_box_2d(h, w):
+    """conv_box: the (h, w) box of at most 128 pixels that covers h x w in the fewest tiles, the wider on a tie"""
     best, th, tw = -1, 1, 1
     for bw in range(1, min(w, 128) + 1):
         bh = min(h, 128 // bw)
@@ -76,7 +77,7 @@ def best_box_2d(h, w):
 
 
 def geometry(op, d):
-    """(output extents on[4], box[4], taps, K, N, input rows) of one entry point, as its TapDesc"""
+    """(output extents on[4], box[4], taps, K, N, input rows) of one entry point, as it fills TapGemmParams"""
     if op in ("linear", "linear_ex"):
         return (d["rows"], 1, 1, 1), (128, 1, 1, 1), 1, d["K"], d["N"], d["rows"]
     if op == "conv2d_3x3":
