@@ -24,6 +24,7 @@ import torch
 import torch.distributed as dist
 
 from ..utils.logger import get_logger
+from ..utils.sharding import _all_gather_owned, _dist_info
 from .solvers_sdedit import sample_dpmpp_2m_sde, sample_heun
 
 logger = get_logger()
@@ -80,45 +81,45 @@ class GaussianDiffusion(object):
         log_var = torch.log(var).clamp_(-20, 20)
 
         out = self._model_out(xt, t, model, model_kwargs, guide_scale, variant_info)
-        if isinstance(out, tuple):
-            x0 = self._guided_x0(out[0], out[1], xt, alphas, sigmas, guide_scale, guide_rescale, clamp, percentile)
-        else:
-            x0 = self._x0_from_out(xt, alphas, sigmas, out, clamp, percentile)
+        x0 = self._x0(xt, out, alphas, sigmas, guide_scale, guide_rescale, clamp, percentile)
         eps = (xt - alphas * x0) / sigmas
         mu = coef1 * x0 + coef2 * xt
         return mu, var, log_var, x0, eps
 
-    def _model_out(self, xt, t, model, model_kwargs, guide_scale, variant_info):
-        """The model call(s) of one denoise evaluation: the output, or the (conditional, unconditional) pair under CFG."""
+    def _model_out(self, xt, t, model, model_kwargs, guide_scale, variant_info, branch=None):
+        """The model call(s) of one denoise evaluation: the output, or the (conditional, unconditional) pair under CFG;
+        ``branch`` (0 = conditional, 1 = unconditional) runs that CFG branch alone (ref :76-88)."""
         if guide_scale is None:
             assert isinstance(model_kwargs, dict)
             return model(xt, t=t, **model_kwargs)
         assert isinstance(model_kwargs, list)
-        pair = getattr(model, "forward_cfg_pair", None)
-        if guide_scale != 1.0 and pair is not None and set(model_kwargs[0]) == set(model_kwargs[1]) == {"y"}:
-            # the two branches differ only in the text embedding: the model evaluates their common, text-independent
-            # prefix once (bit-identical to two calls, tests/test_unet_gpu.py::test_cfg_pair_equals_two_forwards)
-            extra = {}
-            for kw in model_kwargs[2:]:
-                extra.update(kw)
-            if len(model_kwargs) <= 3:
-                extra["variant_info"] = variant_info
-            return pair(xt, t, (model_kwargs[0]["y"], model_kwargs[1]["y"]), **extra)
-        y_out = self._branch_out(xt, t, model, model_kwargs, 0, variant_info)
-        if guide_scale == 1.0:
-            return y_out
-        u_out = self._branch_out(xt, t, model, model_kwargs, 1, variant_info)
-        return (y_out, u_out)
-
-    @staticmethod
-    def _branch_out(xt, t, model, model_kwargs, branch, variant_info):
-        """One CFG branch (0 = conditional, 1 = unconditional) of the model call (ref :76-88)."""
         extra = {}
         for kw in model_kwargs[2:]:
             extra.update(kw)
         if len(model_kwargs) <= 3:
             extra["variant_info"] = variant_info
-        return model(xt, t=t, **model_kwargs[branch], **extra)
+        if branch is not None or guide_scale == 1.0:
+            return model(xt, t=t, **model_kwargs[branch or 0], **extra)
+        pair = getattr(model, "forward_cfg_pair", None)
+        if pair is not None and set(model_kwargs[0]) == set(model_kwargs[1]) == {"y"}:
+            # the two branches differ only in the text embedding: the model evaluates their common, text-independent
+            # prefix once (bit-identical to two calls, tests/test_unet_gpu.py::test_cfg_pair_equals_two_forwards)
+            return pair(xt, t, (model_kwargs[0]["y"], model_kwargs[1]["y"]), **extra)
+        return model(xt, t=t, **model_kwargs[0], **extra), model(xt, t=t, **model_kwargs[1], **extra)
+
+    def _x0(self, xt, out, alphas, sigmas, guide_scale, guide_rescale, clamp=None, percentile=None):
+        """x0 of one evaluation on xt from the model output, or from the (conditional, unconditional) pair under CFG:
+        CFG combine + std-ratio rescale + v -> x0 (ref :89-99).  An fp16 CUDA pair (the .half() UNet) takes the fused
+        device path -- two launches (star_cfg_x0) instead of ~20 eager tensor ops; anything else (CPU tests, fp32 fakes)
+        runs the reference's tensor arithmetic."""
+        if not isinstance(out, tuple):
+            return self._x0_from_out(xt, alphas, sigmas, out, clamp, percentile)
+        y_out, u_out = out
+        if y_out.is_cuda and y_out.dtype == torch.float16 and u_out.dtype == torch.float16 and clamp is None \
+                and percentile is None:
+            from ... import ops
+            return ops.cfg_x0(y_out.contiguous(), u_out.contiguous(), xt, alphas, sigmas, guide_scale, guide_rescale)
+        return self._x0_from_out(xt, alphas, sigmas, self._guided(y_out, u_out, guide_scale, guide_rescale), clamp, percentile)
 
     @staticmethod
     def _x0_from_out(xt, alphas, sigmas, out, clamp=None, percentile=None):
@@ -127,16 +128,6 @@ class GaussianDiffusion(object):
         if clamp is not None or percentile is not None:
             raise NotImplementedError("clamp / percentile are not used on STAR's path (ref video_to_video_model.py:110-123)")
         return alphas * xt - sigmas * out
-
-    def _guided_x0(self, y_out, u_out, xt, alphas, sigmas, guide_scale, guide_rescale, clamp=None, percentile=None):
-        """CFG combine + std-ratio rescale + v -> x0 (ref :89-99).  fp16 CUDA model outputs (the .half() UNet) take
-        the fused device path -- two launches (star_cfg_x0) instead of ~20 eager tensor ops; anything else (CPU tests,
-        fp32 fakes) runs the reference's tensor arithmetic."""
-        if y_out.is_cuda and y_out.dtype == torch.float16 and u_out.dtype == torch.float16 and clamp is None \
-                and percentile is None:
-            from ... import ops
-            return ops.cfg_x0(y_out.contiguous(), u_out.contiguous(), xt, alphas, sigmas, guide_scale, guide_rescale)
-        return self._x0_from_out(xt, alphas, sigmas, self._guided(y_out, u_out, guide_scale, guide_rescale), clamp, percentile)
 
     @staticmethod
     def _guided(y_out, u_out, guide_scale, guide_rescale):
@@ -150,6 +141,11 @@ class GaussianDiffusion(object):
             out = out * (guide_rescale * ratio + (1 - guide_rescale) * 1.0)
         return out
 
+    def _t_coefs(self, xt, sigma):
+        """The timestep of a solver evaluation at k-diffusion ``sigma``, one per sample of xt, and alphas / sigmas there."""
+        t = self._sigma_to_t(sigma).repeat(len(xt)).round().long()
+        return t, _gather_coef(self.alphas, t, xt), _gather_coef(self.sigmas, t, xt)
+
     # -- sampler ---------------------------------------------------------------
     @torch.no_grad()
     def sample_sr(self, noise, model, model_kwargs={}, condition_fn=None, guide_scale=None,
@@ -157,9 +153,10 @@ class GaussianDiffusion(object):
                   solver_mode='fast', steps=20, t_max=None, t_min=None, discretization=None,
                   discard_penultimate_step=None, return_intermediate=None, show_progress=False,
                   seed=-1, chunk_inds=None, variant_info=None, chunk_parallel="auto", tile_inds=None, **kwargs):
-        """``tile_inds`` (the output of video_to_video_model.make_tiles) turns on spatially tiled sampling: every solver-step
-        evaluation runs the model on each (chunk, tile) window and blends the windows' x0 into the clip's x0 with the tiles'
-        weights (see _eval_x0_tiled).  Without it, every path below runs on whole frames."""
+        """Every solver-step evaluation runs the model on the windows of _windows -- the whole clip, or each chunk of
+        ``chunk_inds`` -- and stitches the frames each window keeps into the clip's x0.  ``tile_inds`` (the output of
+        video_to_video_model.make_tiles) turns on spatially tiled sampling: the windows are the (chunk, tile) pairs and
+        their x0 are blended into the clip's x0 with the tiles' weights (see _eval_x0_tiled)."""
         assert isinstance(steps, (int, torch.LongTensor))
         assert t_max is None or (0 < t_max <= self.num_timesteps - 1)
         assert t_min is None or (0 <= t_min < self.num_timesteps - 1)
@@ -179,20 +176,15 @@ class GaussianDiffusion(object):
         # SURVEY App. B); a one-window list is the un-chunked case.
         if chunk_inds is not None and len(chunk_inds) < 2:
             chunk_inds = None
-        if tile_inds is not None and dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
+        if tile_inds is not None and _dist_info()[0] > 1:
             raise NotImplementedError("sample_sr: tiled sampling runs in a single process; spatial tiles are not sharded "
                                       "across ranks")
 
-        intermediates = []
-        world, rank = 1, 0
-        if chunk_inds is not None and chunk_parallel in ("auto", "exact", "literal") \
-                and dist.is_available() and dist.is_initialized():
-            world, rank = dist.get_world_size(), dist.get_rank()
-        mode = "exact" if chunk_parallel == "auto" else chunk_parallel
         # Ranks of one job must integrate the same SDE path -- also for single-chunk clips, where every rank evaluates the whole
         # clip and the pipeline then shards only the VAE legs: share rank 0's noise seed whenever a process group exists.
-        group = (chunk_parallel in ("auto", "exact", "literal") and dist.is_available() and dist.is_initialized()
-                 and dist.get_world_size() > 1)
+        group = chunk_parallel in ("auto", "exact", "literal") and _dist_info()[0] > 1
+        world, rank = _dist_info() if group and chunk_inds is not None else (1, 0)
+        mode = "exact" if chunk_parallel == "auto" else chunk_parallel
         if group and solver == 'dpmpp_2m_sde' and kwargs.get('noise_sampler') is None:
             # every rank applies the same solver update: share the SDE noise stream (rank 0's seed)
             from .solvers_sdedit import IntervalNoiseSampler
@@ -200,46 +192,41 @@ class GaussianDiffusion(object):
             dist.broadcast(sd, 0)
             kwargs['noise_sampler'] = IntervalNoiseSampler(noise, seed=int(sd.item()))
 
+        windows = self._windows(noise, chunk_inds, tile_inds, model_kwargs, guide_scale, clamp, percentile)
+        # CFG-branch split (SURVEY 8e): with at least two ranks per chunk the (chunk, branch) pairs are the units --
+        # BASELINE config 3 (3 chunks) then fills 6 of 8 GPUs instead of 3.
+        split_cfg = (mode == "exact" and world >= 2 * len(windows) and isinstance(model_kwargs, list)
+                     and guide_scale not in (None, 1.0))
+        wire = {}
+        intermediates = []
+
         def eval_x0(xt, sigma, variant_info=None):
-            t = self._sigma_to_t(sigma).repeat(len(xt)).round().long()
-            x0 = self.denoise(xt, t, None, model, model_kwargs, guide_scale, guide_rescale,
-                              clamp, percentile, variant_info=variant_info)[-2]
+            t, alphas, sigmas = self._t_coefs(xt, sigma)
+            if tile_inds is not None:
+                x0 = self._eval_x0_tiled(xt, t, alphas, sigmas, windows, model, model_kwargs, guide_scale, guide_rescale,
+                                         variant_info)
+            elif split_cfg:
+                x0 = self._eval_x0_cfg_split(xt, t, alphas, sigmas, windows, model, model_kwargs, guide_scale,
+                                             guide_rescale, variant_info, world, rank, wire)
+            else:
+                # the kept frames of each window (ref :337-350); in exact mode rank r evaluates windows r, r+W, ...
+                # and ONE all-gather rebuilds the stitched x0 on every rank
+                parts = []
+                for win in windows[rank::world]:
+                    x, out = self._window_out(xt, t, win, model, model_kwargs, guide_scale, variant_info)
+                    lo, hi = win[2:4]
+                    parts.append(self._x0(x, out, alphas, sigmas, guide_scale, guide_rescale, clamp, percentile)[:, :, lo:hi])
+                if world > 1:
+                    b, c, _, h, w = xt.shape
+                    local = torch.concat(parts, dim=2).to(xt.dtype) if parts else xt.new_empty((b, c, 0, h, w))
+                    x0 = _all_gather_owned(local, [hi - lo for _, _, lo, hi, *_ in windows], 2)
+                else:
+                    x0 = torch.concat(parts, dim=2) if len(parts) > 1 else parts[0]
             if return_intermediate == 'xt':
                 intermediates.append(xt)
             elif return_intermediate == 'x0':
                 intermediates.append(x0)
             return x0
-
-        keep = stitch_slices(chunk_inds) if chunk_inds is not None else None
-
-        def chunk_inputs(xt, i):
-            s, e = chunk_inds[i]
-            model_kwargs[2]['hint_chunk'] = model_kwargs[2]['hint'][:, :, s:e].clone()
-            return xt[:, :, s:e].clone()
-
-        def chunk_x0(xt, t, i, variant_info):
-            """x0 of chunk i, cropped to the slice it contributes (ref :337-350)."""
-            x0c = self.denoise(chunk_inputs(xt, i), t, None, model, model_kwargs, guide_scale,
-                               guide_rescale, clamp, percentile, variant_info=variant_info)[-2]
-            lo, hi = keep[i]
-            return x0c[:, :, lo:hi]
-
-        # CFG-branch split (SURVEY 8e): with at least two ranks per chunk the (chunk, branch) pairs are the units --
-        # BASELINE config 3 (3 chunks) then fills 6 of 8 GPUs instead of 3.
-        split_cfg = (world > 1 and chunk_inds is not None and isinstance(model_kwargs, list)
-                     and guide_scale not in (None, 1.0) and world >= 2 * len(chunk_inds)
-                     and chunk_parallel in ("auto", "exact"))
-        wire = {}
-
-        def eval_x0_chunked(xt, sigma, variant_info=None):
-            t = self._sigma_to_t(sigma).repeat(len(xt)).round().long()
-            if world == 1:
-                parts = [chunk_x0(xt, t, i, variant_info) for i in range(len(chunk_inds))]
-                return torch.concat(parts, dim=2)
-            if split_cfg:
-                return self._eval_x0_cfg_split(xt, t, chunk_inds, keep, chunk_inputs, model, model_kwargs, guide_scale,
-                                               guide_rescale, variant_info, world, rank, wire)
-            return self._eval_x0_sharded(xt, t, chunk_inds, keep, chunk_x0, variant_info, world, rank)
 
         # -- timestep / sigma tables (ref :355-406) -----------------------------
         if isinstance(steps, int):
@@ -265,174 +252,126 @@ class GaussianDiffusion(object):
         if discard_penultimate_step:
             sigmas = torch.cat([sigmas[:-2], sigmas[-1:]])
 
-        if tile_inds is not None:
-            windows = self._tile_windows(noise, chunk_inds, keep, tile_inds, model_kwargs, guide_scale, clamp, percentile)
-
-            def eval_x0_tiled(xt, sigma, variant_info=None):
-                t = self._sigma_to_t(sigma).repeat(len(xt)).round().long()
-                x0 = self._eval_x0_tiled(xt, t, windows, model, model_kwargs, guide_scale, guide_rescale, variant_info)
-                if return_intermediate == 'xt':
-                    intermediates.append(xt)
-                elif return_intermediate == 'x0':
-                    intermediates.append(x0)
-                return x0
-            x0 = solver_fn(noise, eval_x0_tiled, sigmas, variant_info=variant_info, show_progress=show_progress, **kwargs)
-        elif chunk_inds is not None and world > 1 and mode == "literal":
-            x0 = self._sample_literal(noise, solver_fn, sigmas, chunk_inds, keep, model, model_kwargs,
-                                      guide_scale, guide_rescale, clamp, percentile, variant_info,
-                                      world, rank, show_progress, kwargs)
+        if world > 1 and mode == "literal":
+            x0 = self._sample_literal(noise, solver_fn, sigmas, windows, model, model_kwargs, guide_scale, guide_rescale,
+                                      clamp, percentile, variant_info, world, rank, show_progress, kwargs)
         else:
-            fn = eval_x0_chunked if chunk_inds is not None else eval_x0
-            x0 = solver_fn(noise, fn, sigmas, variant_info=variant_info, show_progress=show_progress, **kwargs)
+            x0 = solver_fn(noise, eval_x0, sigmas, variant_info=variant_info, show_progress=show_progress, **kwargs)
         return (x0, intermediates) if return_intermediate is not None else x0
 
-    # -- spatially tiled sampling ------------------------------------------------
+    # -- windows: the frames, rows and columns of one model call ---------------------------------------------------------
     @staticmethod
-    def _tile_windows(noise, chunk_inds, keep, tile_inds, model_kwargs, guide_scale, clamp, percentile):
-        """The (chunk, tile) windows of one evaluation: [(s, e, lo, hi, r0, r1, c0, c1, wy, wx)], frames [s, e) of which the
-        chunk keeps [lo, hi) (chunk-local), rows [r0, r1), cols [c0, c1), and the tile's weights uploaded once per call."""
-        if guide_scale is None or not isinstance(model_kwargs, list) or len(model_kwargs) < 3 \
-                or 'hint' not in model_kwargs[2]:
-            raise ValueError("sample_sr(tile_inds=...): tiled sampling needs classifier-free guidance (guide_scale) and "
-                             "model_kwargs [{'y': ...}, {'y': ...}, {'hint': ...}]")
-        if clamp is not None or percentile is not None:
-            raise NotImplementedError("sample_sr(tile_inds=...): clamp / percentile are not supported")
-        rows, cols, row_w, col_w = tile_inds
-        f = noise.shape[2]
-        chunks = chunk_inds if chunk_inds is not None else [(0, f)]
-        kept = keep if keep is not None else [(0, f)]
-        row_w = [w.to(noise.device, torch.float32).contiguous() for w in row_w]
-        col_w = [w.to(noise.device, torch.float32).contiguous() for w in col_w]
+    def _windows(noise, chunk_inds, tile_inds, model_kwargs, guide_scale, clamp, percentile):
+        """The windows of one evaluation: [(s, e, lo, hi, r0, r1, c0, c1, wy, wx)], frames [s, e) of which the x0 keeps
+        [lo, hi) (chunk-local, stitch_slices), rows [r0, r1) and cols [c0, c1).  One whole-frame window per chunk (one for
+        the whole clip without chunks), or one per (chunk, tile) with the tile's weights uploaded once per call (else None)."""
+        f, h, w = noise.shape[2:]
+        chunks, kept = ([(0, f)], [(0, f)]) if chunk_inds is None else (chunk_inds, stitch_slices(chunk_inds))
+        rows, cols, row_w, col_w = [(0, h)], [(0, w)], [None], [None]
+        if tile_inds is not None:
+            if guide_scale is None or not isinstance(model_kwargs, list) or len(model_kwargs) < 3 \
+                    or 'hint' not in model_kwargs[2]:
+                raise ValueError("sample_sr(tile_inds=...): tiled sampling needs classifier-free guidance (guide_scale) and "
+                                 "model_kwargs [{'y': ...}, {'y': ...}, {'hint': ...}]")
+            if clamp is not None or percentile is not None:
+                raise NotImplementedError("sample_sr(tile_inds=...): clamp / percentile are not supported")
+            rows, cols = tile_inds[:2]
+            row_w, col_w = ([v.to(noise.device, torch.float32).contiguous() for v in ws] for ws in tile_inds[2:])
         return [(s, e, lo, hi, r0, r1, c0, c1, wy, wx)
                 for (s, e), (lo, hi) in zip(chunks, kept)
                 for (r0, r1), wy in zip(rows, row_w)
                 for (c0, c1), wx in zip(cols, col_w)]
 
-    def _eval_x0_tiled(self, xt, t, windows, model, model_kwargs, guide_scale, guide_rescale, variant_info):
+    @staticmethod
+    def _crop(x, win):
+        s, e, _, _, r0, r1, c0, c1, _, _ = win
+        return x[:, :, s:e, r0:r1, c0:c1].contiguous()
+
+    def _window_kwargs(self, model_kwargs, win):
+        """The model kwargs of one window: the clip's, with its LR latent cropped to the window as ``hint_chunk``."""
+        return [*model_kwargs[:2], dict(model_kwargs[2], hint_chunk=self._crop(model_kwargs[2]['hint'], win)),
+                *model_kwargs[3:]]
+
+    def _window_out(self, xt, t, win, model, model_kwargs, guide_scale, variant_info, branch=None):
+        """(xt on the window, the model output(s) there; see _model_out).  The model runs on the window's crop of the clip
+        latent and of the LR latent; a window that is the whole clip runs on xt and model_kwargs as they are."""
+        s, e, _, _, r0, r1, c0, c1, _, _ = win
+        if (e - s, r1 - r0, c1 - c0) != tuple(xt.shape[2:]):
+            xt, model_kwargs = self._crop(xt, win), self._window_kwargs(model_kwargs, win)
+        return xt, self._model_out(xt, t, model, model_kwargs, guide_scale, variant_info, branch)
+
+    def _eval_x0_tiled(self, xt, t, alphas, sigmas, windows, model, model_kwargs, guide_scale, guide_rescale, variant_info):
         """x0 of the clip = sum over (chunk, tile) windows of the tile's blend weight times its x0, restricted to the frames
-        the chunk keeps (stitch_slices).  Each window runs the model on the cropped latent and LR latent, with the branch
-        logic of ``denoise``; one star_cfg_x0_blend launch pair per window forms the guided x0 (CFG, std-ratio rescale over
-        the window, v -> x0) and adds it into the clip's x0 in place.  Needs fp16 CUDA model outputs (the .half() UNet)."""
+        the chunk keeps (stitch_slices).  One star_cfg_x0_blend launch pair per window forms the guided x0 (CFG, std-ratio
+        rescale over the window, v -> x0) and adds it into the clip's x0 in place.  Needs fp16 CUDA model outputs (the
+        .half() UNet)."""
         from ... import ops
         xt = xt.float().contiguous()
         x0 = torch.zeros_like(xt)
-        alphas, sigmas = _gather_coef(self.alphas, t, xt), _gather_coef(self.sigmas, t, xt)
-        hint = model_kwargs[2]['hint']                                    # the clip's LR latent; each window gets its crop
-        rescale = None if guide_scale == 1.0 else guide_rescale        # as denoise: no rescale without a second branch
-        for s, e, lo, hi, r0, r1, c0, c1, wy, wx in windows:
-            kw = [model_kwargs[0], model_kwargs[1],
-                  dict(model_kwargs[2], hint_chunk=hint[:, :, s:e, r0:r1, c0:c1].contiguous())] + list(model_kwargs[3:])
-            out = self._model_out(xt[:, :, s:e, r0:r1, c0:c1].contiguous(), t, model, kw, guide_scale, variant_info)
+        rescale = None if guide_scale == 1.0 else guide_rescale        # as _x0: no rescale without a second branch
+        for win in windows:
+            out = self._window_out(xt, t, win, model, model_kwargs, guide_scale, variant_info)[1]
             y_out, u_out = out if isinstance(out, tuple) else (out, out)
             if not (y_out.is_cuda and y_out.dtype == torch.float16 and u_out.dtype == torch.float16):
                 raise TypeError("sample_sr(tile_inds=...): tiled sampling blends on the GPU and needs fp16 CUDA model outputs "
                                 f"(the .half() UNet), got {y_out.dtype} on {y_out.device}")
+            s, _, lo, hi, r0, _, c0, _, wy, wx = win
             ops.cfg_x0(y_out.contiguous(), u_out.contiguous(), xt, alphas, sigmas, guide_scale, rescale,
                        blend=ops.TileBlend(x0, s, lo, hi, r0, c0, wy, wx))
         return x0
 
     # -- chunk-parallel helpers -------------------------------------------------
-    @staticmethod
-    def _eval_x0_sharded(xt, t, chunk_inds, keep, chunk_x0, variant_info, world, rank):
-        """Exact mode: rank r evaluates chunks r, r+W, ...; one all-gather of the
-        kept slices (padded to the longest per-rank payload) rebuilds the
-        stitched x0 on every rank."""
-        n = len(chunk_inds)
-        owner = [i % world for i in range(n)]
-        lens = [hi - lo for lo, hi in keep]
-        per_rank = [sum(l for l, o in zip(lens, owner) if o == r) for r in range(world)]
-        pad = max(per_rank)
-        mine = [chunk_x0(xt, t, i, variant_info) for i in range(n) if owner[i] == rank]
-        b, c, _, h, w = xt.shape
-        send = xt.new_zeros((b, c, pad, h, w))
-        if mine:
-            cat = torch.concat(mine, dim=2)
-            send[:, :, :cat.shape[2]] = cat.to(send.dtype)
-        recv = [torch.empty_like(send) for _ in range(world)]
-        dist.all_gather(recv, send.contiguous())
-        cursor = [0] * world
-        parts = []
-        for i in range(n):
-            r = owner[i]
-            parts.append(recv[r][:, :, cursor[r]:cursor[r] + lens[i]])
-            cursor[r] += lens[i]
-        return torch.concat(parts, dim=2)
-
-    def _eval_x0_cfg_split(self, xt, t, chunk_inds, keep, chunk_inputs, model, model_kwargs, guide_scale, guide_rescale,
+    def _eval_x0_cfg_split(self, xt, t, alphas, sigmas, windows, model, model_kwargs, guide_scale, guide_rescale,
                            variant_info, world, rank, wire):
         """Exact mode with two ranks per chunk: rank 2i evaluates the conditional branch of chunk i, rank 2i+1 the
         unconditional one (ranks >= 2n idle).  ONE all-gather of the raw model outputs per solver step; every rank
         then forms the guided output (needs both branches: std-ratio rescale, ref :89-97), x0 and the stitch for all
         chunks -- elementwise work on a few MB, identical on every rank and to the serial loop."""
-        n = len(chunk_inds)
-        lens = [e - s for s, e in chunk_inds]
         b, c, _, h, w = xt.shape
         out = None
-        if rank < 2 * n:
+        if rank < 2 * len(windows):
             i, branch = divmod(rank, 2)
-            out = self._branch_out(chunk_inputs(xt, i), t, model, model_kwargs, branch, variant_info)
+            out = self._window_out(xt, t, windows[i], model, model_kwargs, guide_scale, variant_info, branch)[1]
         if "dtype" not in wire:                      # the model's output dtype (fp16 for the .half() UNet), agreed once
             codes = [torch.float16, torch.bfloat16, torch.float32, torch.float64]
             code = torch.tensor([codes.index(out.dtype) if out is not None else 0], device=xt.device)
             dist.broadcast(code, 0)
             wire["dtype"] = codes[int(code.item())]
-        send = torch.zeros((b, c, max(lens), h, w), dtype=wire["dtype"], device=xt.device)
+        send = torch.zeros((b, c, max(e - s for s, e, *_ in windows), h, w), dtype=wire["dtype"], device=xt.device)
         if out is not None:
             send[:, :, :out.shape[2]] = out
         recv = [torch.empty_like(send) for _ in range(world)]
         dist.all_gather(recv, send)
-        sig = _gather_coef(self.sigmas, t, xt)
-        alp = _gather_coef(self.alphas, t, xt)
         parts = []
-        for i, (s, e) in enumerate(chunk_inds):
-            y_out, u_out = recv[2 * i][:, :, :lens[i]], recv[2 * i + 1][:, :, :lens[i]]
-            x0c = self._guided_x0(y_out, u_out, xt[:, :, s:e], alp, sig, guide_scale, guide_rescale)
-            lo, hi = keep[i]
+        for (s, e, lo, hi, *_), y_out, u_out in zip(windows, recv[0::2], recv[1::2]):
+            x0c = self._x0(xt[:, :, s:e], (y_out[:, :, :e - s], u_out[:, :, :e - s]), alphas, sigmas, guide_scale,
+                           guide_rescale)
             parts.append(x0c[:, :, lo:hi])
         return torch.concat(parts, dim=2)
 
-    def _sample_literal(self, noise, solver_fn, sigmas, chunk_inds, keep, model, model_kwargs, guide_scale,
-                        guide_rescale, clamp, percentile, variant_info, world, rank, show_progress, kwargs):
+    def _sample_literal(self, noise, solver_fn, sigmas, windows, model, model_kwargs, guide_scale, guide_rescale, clamp,
+                        percentile, variant_info, world, rank, show_progress, kwargs):
         """North-star literal mode: every rank integrates its own chunk(s) for
         all solver steps with no exchange; kept slices are gathered once."""
-        n = len(chunk_inds)
-        b, c, f, h, w = noise.shape
-        lens = [hi - lo for lo, hi in keep]
-        owner = [i % world for i in range(n)]
-        per_rank = [sum(l for l, o in zip(lens, owner) if o == r) for r in range(world)]
-        pad = max(per_rank)
         outs = []
-        for i in range(n):
-            if owner[i] != rank:
-                continue
-            s, e = chunk_inds[i]
-            kw = [model_kwargs[0], model_kwargs[1], {'hint': model_kwargs[2]['hint'][:, :, s:e].clone()}]
+        for win in windows[rank::world]:
+            s, e, lo, hi = win[:4]
+            kw = self._window_kwargs(model_kwargs, win)
 
             def fn(xt, sigma, variant_info=None, kw=kw):
-                t = self._sigma_to_t(sigma).repeat(len(xt)).round().long()
-                return self.denoise(xt, t, None, model, kw, guide_scale, guide_rescale, clamp, percentile,
-                                    variant_info=variant_info)[-2]
+                t, al, sg = self._t_coefs(xt, sigma)
+                out = self._model_out(xt, t, model, kw, guide_scale, variant_info)
+                return self._x0(xt, out, al, sg, guide_scale, guide_rescale, clamp, percentile)
             kw_i = dict(kwargs)
             if kw_i.get('noise_sampler') is not None:       # injected full-clip noise: use this chunk's frames
                 full = kw_i['noise_sampler']
                 kw_i['noise_sampler'] = lambda a, b, full=full, s=s, e=e: full(a, b)[:, :, s:e]
             xi = solver_fn(noise[:, :, s:e].clone(), fn, sigmas, variant_info=variant_info,
                            show_progress=show_progress, **kw_i)
-            lo, hi = keep[i]
             outs.append(xi[:, :, lo:hi])
-        send = noise.new_zeros((b, c, pad, h, w))
-        if outs:
-            cat = torch.concat(outs, dim=2)
-            send[:, :, :cat.shape[2]] = cat
-        recv = [torch.empty_like(send) for _ in range(world)]
-        dist.all_gather(recv, send.contiguous())
-        cursor = [0] * world
-        parts = []
-        for i in range(n):
-            r = owner[i]
-            parts.append(recv[r][:, :, cursor[r]:cursor[r] + lens[i]])
-            cursor[r] += lens[i]
-        return torch.concat(parts, dim=2)
+        b, c, _, h, w = noise.shape
+        local = torch.concat(outs, dim=2).to(noise.dtype) if outs else noise.new_empty((b, c, 0, h, w))
+        return _all_gather_owned(local, [hi - lo for _, _, lo, hi, *_ in windows], 2)
 
     # -- sigma <-> t in k-diffusion space (ref :415-443) ---------------------------
     def _log_kd_sigmas(self, like):

@@ -32,42 +32,11 @@ from .diffusion.schedules_sdedit import noise_schedule
 from .modules.unet_v2v import ControlledV2VUNet, rearrange
 from .utils.config import cfg
 from .utils.logger import get_logger
+from .utils.sharding import _all_gather_owned, _all_gather_varlen, _dist_info, _shard_bounds
 
 logger = get_logger()
 
 __all__ = ["VideoToVideo_sr", "pad_to_fit", "make_chunks", "make_tiles", "sliding_windows_1d"]
-
-
-def _dist_info():
-    if dist.is_available() and dist.is_initialized():
-        return dist.get_world_size(), dist.get_rank()
-    return 1, 0
-
-
-def _shard_bounds(n, world):
-    """contiguous, balanced split of n items over `world` ranks: [(lo, hi)] (empty shards when n < world)"""
-    base, extra = divmod(n, world)
-    out, lo = [], 0
-    for r in range(world):
-        hi = lo + base + (1 if r < extra else 0)
-        out.append((lo, hi))
-        lo = hi
-    return out
-
-
-def _all_gather_varlen(local, counts, dim):
-    """all-gather of per-rank tensors whose extent along `dim` is counts[rank] (padded to the longest share);
-    returns the concatenation in rank order.  ONE collective."""
-    world, rank = _dist_info()
-    pad = max(counts)
-    shape = list(local.shape)
-    shape[dim] = pad
-    send = local.new_zeros(shape)
-    if counts[rank]:
-        send.narrow(dim, 0, counts[rank]).copy_(local)
-    recv = [torch.empty_like(send) for _ in range(world)]
-    dist.all_gather(recv, send)
-    return torch.cat([recv[r].narrow(dim, 0, counts[r]) for r in range(world) if counts[r]], dim=dim)
 
 
 class VideoToVideo_sr():
@@ -255,7 +224,6 @@ class VideoToVideo_sr():
         starts = list(range(0, n, chunk_size))
         mine = starts[rank::world]
         outs = [self.temporal_vae_decode(zf[s:s + chunk_size], min(chunk_size, n - s))[:, :, t0:t1, l0:l1] for s in mine]
-        counts = [sum(min(chunk_size, n - s) for s in starts[r::world]) for r in range(world)]
         if outs:
             local = torch.cat(outs)
         else:
@@ -263,17 +231,7 @@ class VideoToVideo_sr():
         dtype_code = torch.tensor([0 if local.dtype == torch.float16 else 1], device=self.device)
         dist.all_reduce(dtype_code, op=dist.ReduceOp.MAX)
         local = local.to(torch.float16 if int(dtype_code.item()) == 0 else torch.float32)
-        gathered = _all_gather_varlen(local, counts, 0)                   # rank-major: windows r, r+W, ... of rank r
-        order, pos = [], 0
-        frame_of = {}
-        for r in range(world):
-            for s in starts[r::world]:
-                k = min(chunk_size, n - s)
-                for j in range(k):
-                    frame_of[s + j] = pos + j
-                pos += k
-        idx = torch.tensor([frame_of[f] for f in range(n)], device=gathered.device)
-        return gathered.index_select(0, idx)
+        return _all_gather_owned(local, [min(chunk_size, n - s) for s in starts], 0)
 
     # -- VAE helpers (ref :141-161): exact 3-frame decode windows, 1-frame encode ----------------------
     def temporal_vae_decode(self, z, num_f):
