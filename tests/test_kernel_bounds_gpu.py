@@ -41,6 +41,12 @@ ERR_ERF_AS = 1.5e-7 + 2.0 ** -22     # erf_as: Abramowitz-Stegun 7.1.26 (|err| <
 ERR_TANH_APPROX = 2.0 ** -10.9       # tanh.approx.f32: about 2^-11 relative (PTX ISA), |tanh| <= 1 so also absolute
 ERR_EX2 = 2.0 ** -22                 # ex2.approx.ftz.f32: relative error (PTX ISA: 2^-22.5 and better); also __expf's core
 SUBNORMAL_P = 2.0 ** -25  # fp16 P: weights below 2^-14 round with absolute error up to half the smallest subnormal
+# Which weights can be subnormal: the kernel rounds p = 2^(s log2e - m) against its running maximum m, which never exceeds the
+# final one, so p >= e (1 - d) where e = exp(s - max s) is the reference weight and d <= K_SCORE / 2 U32 scale |q||k| + ERR_EX2
+# its relative error (the score term below, and ex2.approx).  Only keys with e < 2^-14 / (1 - d) can round as subnormals, and
+# 1 / (1 - d) <= 1 + 2 d for d <= 1/2, so the term sums |v| over e < 2^-14 (1 + SUBNORMAL_MARGIN d).  Their absolute errors
+# sit in the unnormalised accumulator (rescaled by alpha <= 1 afterwards) and are divided by l >= 1 like the rest of it.
+SUBNORMAL_MARGIN = 2
 # Score error: 4 k16 steps over head_dim 64 at ROUND_PER_K16 each, plus the fp32 scale*log2e multiply and the fmaf against the
 # running max (relative to |s|, itself <= |q||k|); a relative error e of every softmax weight moves the output by <= 2 e (P|V|).
 K_SCORE = 2 * (4 * ROUND_PER_K16 + 6)
@@ -67,24 +73,26 @@ class BoundCheck:
         self.what, self.family, self.locate, self.nshow = what, family, locate, nshow
         self.worst, self.worst_at, self.nbad, self.shown, self.n = 0.0, None, 0, [], 0
 
-    def add(self, got, y, bound, row0=0):
+    def add(self, got, y, bound, row0=0, rows=None, col0=0):
+        """rows (optional): the global row index of every local row, for chunks that are not a contiguous row range"""
         assert got.shape == y.shape == bound.shape, f"{self.what}: shapes {tuple(got.shape)} {tuple(y.shape)} {tuple(bound.shape)}"
+        at = lambda r, c: (int(rows[r]) if rows is not None else r + row0, c + col0)       # noqa: E731
         g = got.to(F64)
         if not torch.isfinite(g).all():
             bad = (~torch.isfinite(g)).nonzero()[: self.nshow].tolist()
-            raise AssertionError(f"{self.what}: non-finite output at (row, col) {[(r + row0, c) for r, c in bad]}")
+            raise AssertionError(f"{self.what}: non-finite output at (row, col) {[at(r, c) for r, c in bad]}")
         ratio = (g - y).abs() / bound
         self.n += ratio.numel()
         w = ratio.max().item()
         if w > self.worst:
             flat = int(ratio.argmax().item())
-            self.worst, self.worst_at = w, (flat // ratio.shape[1] + row0, flat % ratio.shape[1])
+            self.worst, self.worst_at = w, at(flat // ratio.shape[1], flat % ratio.shape[1])
         badmask = ratio > 1.0
         nb = int(badmask.sum().item())
         if nb:
             self.nbad += nb
             for r, c in badmask.nonzero()[: max(0, self.nshow - len(self.shown))].tolist():
-                self.shown.append((r + row0, c, g[r, c].item(), y[r, c].item(), bound[r, c].item()))
+                self.shown.append((*at(r, c), g[r, c].item(), y[r, c].item(), bound[r, c].item()))
         return self
 
     def done(self):
@@ -155,22 +163,31 @@ def tap_epilogue(acc, mag, k16_steps, dtype, bias=None, geglu=False, act=None, c
     return y, _finish(y, err, dtype)
 
 
-def attention_core(q, k, v, scale, dtype, causal=False):
+def attention_core(q, k, v, scale, dtype, causal=False, q0=0):
     """fp64 softmax(q k^T scale) v over [..., N, 64] and its bound.  Kernel error: the scores (K_SCORE), ex2.approx of every
     weight, P rounded to the storage type before the P V MMA while l sums the unrounded weights (2 u_p), the fp32 P V and l
-    accumulations, fp16 P subnormals; all relative to P|V| except the last."""
-    s = (q @ k.transpose(-1, -2)) * scale
+    accumulations, fp16 P subnormals; all relative to P|V| except the last.  q0: sequence index of the first query row (a
+    row chunk of a causal problem)."""
+    s = (q @ k.transpose(-1, -2)).mul_(scale)
     nq, nk = s.shape[-2], s.shape[-1]
     if causal:
-        s = s.masked_fill(torch.ones(nq, nk, dtype=torch.bool, device=s.device).triu(1), float("-inf"))
-    e = torch.exp(s - s.amax(-1, keepdim=True))
-    p = e / e.sum(-1, keepdim=True)
-    y = p @ v
-    pv = p @ v.abs()
+        qidx = q0 + torch.arange(nq, device=s.device)
+        s.masked_fill_(torch.arange(nk, device=s.device)[None, :] > qidx[:, None], float("-inf"))
+    e = s.sub_(s.amax(-1, keepdim=True)).exp_()
+    l = e.sum(-1, keepdim=True)
+    va = v.abs()
     qk = q.norm(dim=-1, keepdim=True) * k.norm(dim=-1).amax(-1, keepdim=True).unsqueeze(-1)
+    score = K_SCORE * U32 * scale * qk
+    sub = None
+    if dtype == HALF:
+        sub = ((e < 2.0 ** -14 * (1 + SUBNORMAL_MARGIN * (score / 2 + ERR_EX2))).to(F64) @ va) / l
+    p = e.div_(l)
+    y = p @ v
+    pv = p @ va
+    del s, e, p
     u_p = U_OUT[dtype]
-    rel = 2 * u_p + 2 * ERR_EX2 + U32 * (ROUND_PER_K16 * _ceil(nk, 16) + _ceil(nk, 4) + 8) + K_SCORE * U32 * scale * qk
-    err = rel * pv + (SUBNORMAL_P if dtype == HALF else 0.0) * v.abs().sum(-2, keepdim=True)
+    rel = 2 * u_p + 2 * ERR_EX2 + U32 * (ROUND_PER_K16 * _ceil(nk, 16) + _ceil(nk, 4) + 8) + score
+    err = rel * pv if sub is None else rel * pv + SUBNORMAL_P * sub
     return y, _finish(y, err, dtype)
 
 
