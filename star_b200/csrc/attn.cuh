@@ -6,12 +6,9 @@
 //
 // One CTA = 128 query rows of one (batch, head).  Warp roles (384 threads):
 //   warpgroup 0      one TMA producer thread: Q once, then K/V tiles (128 keys) through a ring of stages
-//   warpgroups 1, 2  64 query rows each:
-//                      S_j = Q K_j^T            wgmma m64n128k16, both operands K-major in shared memory
-//                      online softmax on the S fragment in registers (two rows per thread, quad shuffles)
-//                      O  += P_j V_j            wgmma m64n64k16 with P as the register A operand (the S
-//                                               accumulator fragment packed to fp16 pairs) and V MN-major
+//   warpgroups 1, 2  64 query rows each, one attn_block_step<128> per K/V tile
 // Keys beyond Nk are zero-filled by TMA and masked; with `causal` the key tiles past the last query row are skipped.
+// attn_block_step is also the consumer step of temporal_attn_long_kernel (tattn_long.cuh).
 #pragma once
 #include "common.cuh"
 #include "wgmma.cuh"
@@ -43,15 +40,87 @@ struct AttnSmem {
     static constexpr int TOTAL = OFF_BAR + 256 + 1024;
 };
 
+// One key block of a consumer warpgroup's online softmax over 64 query rows, for the thread's two rows h of the
+// accumulator fragment (wgmma.cuh):
+//     S = Q K^T     over the BKV keys from kbase, wgmma m64nBKVk16, both operands K-major in shared memory
+//     softmax       keys at or past klim[h] masked; running max m_run (scaled, log2 domain) and sum l_run updated with
+//                   quad shuffles, O rescaled
+//     O += P V      wgmma m64n64k16 with P as the register A operand (the S fragment packed to pairs), V MN-major
+template <int BKV>
+STAR_DEVINL void attn_block_step(float (&o)[32], float (&m_run)[2], float (&l_run)[2], uint64_t dq, uint64_t dk,
+                                 uint64_t dv, int kbase, const int (&klim)[2], float sl2) {
+    static_assert(BKV == 64 || BKV == 128, "key blocks of 64 or 128");
+    const int q4 = threadIdx.x & 3;
+    float sacc[BKV / 2];
+#pragma unroll
+    for (int i = 0; i < BKV / 2; ++i) sacc[i] = 0.f;
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < AT_D / 16; ++k) {
+        if constexpr (BKV == 128) wgmma_m64n128_ss(sacc, dq + 2 * k, dk + 2 * k);
+        else wgmma_m64n64_ss(sacc, dq + 2 * k, dk + 2 * k);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+
+    float alpha[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        if (kbase + BKV > klim[h]) {
+#pragma unroll
+            for (int jj = 0; jj < BKV / 8; ++jj)
+#pragma unroll
+                for (int e = 0; e < 2; ++e)
+                    if (kbase + 8 * jj + 2 * q4 + e >= klim[h]) sacc[4 * jj + 2 * h + e] = -INFINITY;
+        }
+        float mx = -INFINITY;
+#pragma unroll
+        for (int jj = 0; jj < BKV / 8; ++jj) mx = fmaxf(mx, fmaxf(sacc[4 * jj + 2 * h], sacc[4 * jj + 2 * h + 1]));
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+        const float m_new = fmaxf(m_run[h], mx * sl2);
+        alpha[h] = ex2_approx(m_run[h] - m_new);
+        m_run[h] = m_new;
+        float l = 0.f;
+#pragma unroll
+        for (int jj = 0; jj < BKV / 8; ++jj)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const float pv = ex2_approx(fmaf(sacc[4 * jj + 2 * h + e], sl2, -m_new));
+                sacc[4 * jj + 2 * h + e] = pv;
+                l += pv;
+            }
+        l_run[h] = l_run[h] * alpha[h] + l;
+    }
+    // P as the A operand of P V: k-step kk covers keys [16 kk, 16 kk + 16) = accumulator columns of pairs 2kk, 2kk+1
+    uint32_t pa[BKV / 16][4];
+#pragma unroll
+    for (int kk = 0; kk < BKV / 16; ++kk) {
+        pa[kk][0] = pack_half2(sacc[8 * kk + 0], sacc[8 * kk + 1]);
+        pa[kk][1] = pack_half2(sacc[8 * kk + 2], sacc[8 * kk + 3]);
+        pa[kk][2] = pack_half2(sacc[8 * kk + 4], sacc[8 * kk + 5]);
+        pa[kk][3] = pack_half2(sacc[8 * kk + 6], sacc[8 * kk + 7]);
+    }
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {
+        o[4 * jj + 0] *= alpha[0];
+        o[4 * jj + 1] *= alpha[0];
+        o[4 * jj + 2] *= alpha[1];
+        o[4 * jj + 3] *= alpha[1];
+    }
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < BKV / 16; ++kk) wgmma_m64n64_rs_tb(o, pa[kk], dv + (uint64_t)(kk * (2048 >> 4)));
+    wgmma_commit();
+    wgmma_wait<0>();
+}
+
 __global__ void __launch_bounds__(AT_THREADS, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                 const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ AttnParams p) {
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + AttnSmem::OFF_BAR);
-    uint64_t* q_full = bars;                           // 1
-    uint64_t* kv_full = bars + 1;                      // AT_KV_STAGES
-    uint64_t* kv_empty = kv_full + AT_KV_STAGES;       // AT_KV_STAGES
+    uint8_t* smem = dyn_smem_1024();
+    uint64_t* q_full = reinterpret_cast<uint64_t*>(smem + AttnSmem::OFF_BAR);
+    StageRing<AT_KV_STAGES> kv(q_full + 1);
 
     const int wg = threadIdx.x >> 7;
     const int warp = threadIdx.x >> 5;
@@ -68,10 +137,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
         tma_prefetch_desc(&tmap_k);
         tma_prefetch_desc(&tmap_v);
         mbar_init(q_full, 1);
-        for (int s = 0; s < AT_KV_STAGES; ++s) {
-            mbar_init(&kv_full[s], 1);
-            mbar_init(&kv_empty[s], AT_CONSUMER_WARPS);
-        }
+        kv.init(AT_CONSUMER_WARPS);
         fence_barrier_init();
     }
     __syncthreads();
@@ -81,14 +147,13 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
         if (threadIdx.x == 0) {
             mbar_expect_tx(q_full, AttnSmem::TILE);
             tma_load_3d(smem + AttnSmem::OFF_Q, &tmap_q, q_full, head * AT_D, q0, batch);
-            int s = 0;
-            uint32_t ph = 0;
             for (int j = 0; j < nt; ++j) {
-                mbar_wait(&kv_empty[s], ph ^ 1);
-                mbar_expect_tx(&kv_full[s], 2 * AttnSmem::TILE);
-                tma_load_3d(smem + AttnSmem::OFF_K + s * AttnSmem::TILE, &tmap_k, &kv_full[s], head * AT_D, j * AT_BKV, kv_batch);
-                tma_load_3d(smem + AttnSmem::OFF_V + s * AttnSmem::TILE, &tmap_v, &kv_full[s], head * AT_D, j * AT_BKV, kv_batch);
-                if (++s == AT_KV_STAGES) { s = 0; ph ^= 1; }
+                kv.wait_empty();
+                uint64_t* full = &kv.full[kv.s];
+                mbar_expect_tx(full, 2 * AttnSmem::TILE);
+                tma_load_3d(smem + AttnSmem::OFF_K + kv.s * AttnSmem::TILE, &tmap_k, full, head * AT_D, j * AT_BKV, kv_batch);
+                tma_load_3d(smem + AttnSmem::OFF_V + kv.s * AttnSmem::TILE, &tmap_v, full, head * AT_D, j * AT_BKV, kv_batch);
+                kv.advance();
             }
         }
         return;
@@ -99,11 +164,12 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
     const int q4 = lane & 3;
     const int row_in_wg = (warp & 3) * 16 + (lane >> 2);
     const int qrow[2] = {q0 + cw * 64 + row_in_wg, q0 + cw * 64 + row_in_wg + 8};
+    const int klim[2] = {p.causal ? min(p.Nk, qrow[0] + 1) : p.Nk,           // keys [0, klim) are visible to the row
+                         p.causal ? min(p.Nk, qrow[1] + 1) : p.Nk};
     const uint64_t dq = wgmma_desc_sw128(smem_u32(smem + AttnSmem::OFF_Q) + cw * 64 * 128, 16, 1024);
     const uint64_t dk0 = wgmma_desc_sw128(smem_u32(smem + AttnSmem::OFF_K), 16, 1024);
     const uint64_t dv0 = wgmma_desc_sw128(smem_u32(smem + AttnSmem::OFF_V), 8192, 1024);
     constexpr uint64_t TILE_INC = (uint64_t)(AttnSmem::TILE >> 4);
-    const float sl2 = p.scale_log2;
 
     float o[32];
 #pragma unroll
@@ -111,76 +177,13 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
     float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
 
     mbar_wait(q_full, 0);
-    int s = 0;
-    uint32_t ph = 0;
 #pragma unroll 1
     for (int j = 0; j < nt; ++j) {
-        mbar_wait(&kv_full[s], ph);
-        float sacc[64];
-#pragma unroll
-        for (int i = 0; i < 64; ++i) sacc[i] = 0.f;
-        const uint64_t dk = dk0 + TILE_INC * (uint64_t)s;
-        wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < AT_D / 16; ++k) wgmma_m64n128_ss(sacc, dq + 2 * k, dk + 2 * k);
-        wgmma_commit();
-        wgmma_wait<0>();
-
-        const int kbase = j * AT_BKV;
-        float alpha[2];
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-            const int klim = p.causal ? min(p.Nk, qrow[h] + 1) : p.Nk;     // keys [0, klim) are visible to this row
-            float mx = -INFINITY;
-            if (kbase + AT_BKV > klim) {
-#pragma unroll
-                for (int jj = 0; jj < 16; ++jj)
-#pragma unroll
-                    for (int e = 0; e < 2; ++e)
-                        if (kbase + 8 * jj + 2 * q4 + e >= klim) sacc[4 * jj + 2 * h + e] = -INFINITY;
-            }
-#pragma unroll
-            for (int jj = 0; jj < 16; ++jj) mx = fmaxf(mx, fmaxf(sacc[4 * jj + 2 * h], sacc[4 * jj + 2 * h + 1]));
-            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
-            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
-            const float m_new = fmaxf(m_run[h], mx * sl2);
-            alpha[h] = ex2_approx(m_run[h] - m_new);
-            m_run[h] = m_new;
-            float l = 0.f;
-#pragma unroll
-            for (int jj = 0; jj < 16; ++jj)
-#pragma unroll
-                for (int e = 0; e < 2; ++e) {
-                    const float pv = ex2_approx(fmaf(sacc[4 * jj + 2 * h + e], sl2, -m_new));
-                    sacc[4 * jj + 2 * h + e] = pv;
-                    l += pv;
-                }
-            l_run[h] = l_run[h] * alpha[h] + l;
-        }
-        // P as the A operand of P V: k-step kk covers keys [16 kk, 16 kk + 16) = accumulator columns of pairs 2kk, 2kk+1
-        uint32_t pa[AT_BKV / 16][4];
-#pragma unroll
-        for (int kk = 0; kk < AT_BKV / 16; ++kk) {
-            pa[kk][0] = pack_half2(sacc[8 * kk + 0], sacc[8 * kk + 1]);
-            pa[kk][1] = pack_half2(sacc[8 * kk + 2], sacc[8 * kk + 3]);
-            pa[kk][2] = pack_half2(sacc[8 * kk + 4], sacc[8 * kk + 5]);
-            pa[kk][3] = pack_half2(sacc[8 * kk + 6], sacc[8 * kk + 7]);
-        }
-#pragma unroll
-        for (int jj = 0; jj < 8; ++jj) {
-            o[4 * jj + 0] *= alpha[0];
-            o[4 * jj + 1] *= alpha[0];
-            o[4 * jj + 2] *= alpha[1];
-            o[4 * jj + 3] *= alpha[1];
-        }
-        const uint64_t dv = dv0 + TILE_INC * (uint64_t)s;
-        wgmma_fence();
-#pragma unroll
-        for (int kk = 0; kk < AT_BKV / 16; ++kk) wgmma_m64n64_rs_tb(o, pa[kk], dv + (uint64_t)(kk * (2048 >> 4)));
-        wgmma_commit();
-        wgmma_wait<0>();
-        if (lane == 0) mbar_arrive(&kv_empty[s]);
-        if (++s == AT_KV_STAGES) { s = 0; ph ^= 1; }
+        kv.wait_full();
+        attn_block_step<AT_BKV>(o, m_run, l_run, dq, dk0 + TILE_INC * (uint64_t)kv.s, dv0 + TILE_INC * (uint64_t)kv.s,
+                                j * AT_BKV, klim, p.scale_log2);
+        kv.release(kv.s);
+        kv.advance();
     }
 
 #pragma unroll

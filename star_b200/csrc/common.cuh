@@ -75,6 +75,44 @@ STAR_DEVINL void mbar_wait(uint64_t* bar, uint32_t parity) {
     }
 }
 
+// A ring of NS shared-memory stages between one TMA producer thread and the consumer warps.  Stage s has a full
+// barrier (the producer's expect_tx, completed by the TMA bytes) and an empty barrier (one arrive per consumer warp),
+// full[0..NS) followed by empty[0..NS).  The producer and every consumer thread each keep their own position and walk
+// the stages in the same order.  A stage's n-th use completes phase n of its full barrier and, once released, phase n of
+// its empty barrier.  So for use n a consumer waits for full at parity n & 1, and the producer waits for phase n - 1 of
+// empty, at the opposite parity, which a freshly initialised barrier passes: the first lap needs no release.
+template <int NS>
+struct StageRing {
+    uint64_t* full;
+    uint64_t* empty;
+    int s = 0;           // current stage
+    uint32_t ph = 0;     // parity of the current lap
+
+    STAR_DEVINL explicit StageRing(uint64_t* bars) : full(bars), empty(bars + NS) {}
+    STAR_DEVINL void init(uint32_t consumer_warps) const {       // thread 0, before the CTA-wide barrier-init fence
+        for (int i = 0; i < NS; ++i) {
+            mbar_init(&full[i], 1);
+            mbar_init(&empty[i], consumer_warps);
+        }
+    }
+    STAR_DEVINL void wait_empty() const { mbar_wait(&empty[s], ph ^ 1); }
+    STAR_DEVINL void wait_full() const { mbar_wait(&full[s], ph); }
+    // Called by every thread of a consumer warp once its reads of the stage are complete.
+    STAR_DEVINL void release(int stage) const {
+        if ((threadIdx.x & 31) == 0) mbar_arrive(&empty[stage]);
+    }
+    STAR_DEVINL void advance() {
+        if (++s == NS) { s = 0; ph ^= 1; }
+    }
+};
+
+// Dynamic shared memory rounded up to 1024 B, the alignment of 128-byte-swizzled TMA tiles and wgmma operands: kernels
+// that use it request 1 KB more than their layout needs.
+STAR_DEVINL uint8_t* dyn_smem_1024() {
+    extern __shared__ uint8_t smem_raw[];
+    return reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+}
+
 // ---------------------------------------------------------------- fences
 STAR_DEVINL void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 

@@ -253,11 +253,8 @@ __global__ void __launch_bounds__(TG_THREADS, 1)
 tapgemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_w,
                const __grid_constant__ TapGemmParams p) {
     using SM = TapGemmSmem<BN>;
-    constexpr int NS = SM::STAGES;
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + NS * SM::STAGE_BYTES);
-    uint64_t* empty_bar = full_bar + NS;
+    uint8_t* smem = dyn_smem_1024();
+    StageRing<SM::STAGES> ring(reinterpret_cast<uint64_t*>(smem + SM::STAGES * SM::STAGE_BYTES));
 
     const int wg = threadIdx.x >> 7;
     const int warp = threadIdx.x >> 5;
@@ -268,10 +265,7 @@ tapgemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
     if (threadIdx.x == 0) {
         tma_prefetch_desc(&tmap_a);
         tma_prefetch_desc(&tmap_w);
-        for (int s = 0; s < NS; ++s) {
-            mbar_init(&full_bar[s], 1);
-            mbar_init(&empty_bar[s], TG_CONSUMER_WARPS);
-        }
+        ring.init(TG_CONSUMER_WARPS);
         fence_barrier_init();
     }
     __syncthreads();
@@ -291,8 +285,6 @@ tapgemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
         asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
         if (threadIdx.x == 0) {
             const uint32_t tx = (uint32_t)p.box_rows * 128u + (uint32_t)SM::B_BYTES;
-            int s = 0;
-            uint32_t ph = 0;
             for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
                 int org[4], n_tile;
                 tile_origin(tile, org, n_tile);
@@ -300,19 +292,20 @@ tapgemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
                     const int c1 = org[0] + p.tap[t][0], c2 = org[1] + p.tap[t][1];
                     const int c3 = org[2] + p.tap[t][2], c4 = org[3] + p.tap[t][3];
                     for (int kc = 0; kc < p.k_chunks; ++kc) {
-                        mbar_wait(&empty_bar[s], ph ^ 1);
-                        uint8_t* sa = smem + s * SM::STAGE_BYTES;
+                        ring.wait_empty();
+                        uint64_t* full = &ring.full[ring.s];
+                        uint8_t* sa = smem + ring.s * SM::STAGE_BYTES;
                         uint8_t* sb = sa + SM::A_BYTES;
-                        mbar_expect_tx(&full_bar[s], tx);
-                        tma_load_5d(sa, &tmap_a, &full_bar[s], kc * TG_BK, c1, c2, c3, c4);
+                        mbar_expect_tx(full, tx);
+                        tma_load_5d(sa, &tmap_a, full, kc * TG_BK, c1, c2, c3, c4);
                         const int kw = t * p.K + kc * TG_BK;
                         if (!geglu) {
-                            tma_load_2d(sb, &tmap_w, &full_bar[s], kw, n_tile * BN);
+                            tma_load_2d(sb, &tmap_w, full, kw, n_tile * BN);
                         } else {
-                            tma_load_2d(sb, &tmap_w, &full_bar[s], kw, n_tile * (BN / 2));
-                            tma_load_2d(sb + (BN / 2) * 128, &tmap_w, &full_bar[s], kw, p.N + n_tile * (BN / 2));
+                            tma_load_2d(sb, &tmap_w, full, kw, n_tile * (BN / 2));
+                            tma_load_2d(sb + (BN / 2) * 128, &tmap_w, full, kw, p.N + n_tile * (BN / 2));
                         }
-                        if (++s == NS) { s = 0; ph ^= 1; }
+                        ring.advance();
                     }
                 }
             }
@@ -328,8 +321,6 @@ tapgemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
     const uint64_t desc_a0 = wgmma_desc_sw128(smem_u32(smem) + cw * 64 * 128, 16, 1024);
     const uint64_t desc_b0 = wgmma_desc_sw128(smem_u32(smem) + SM::A_BYTES, 16, 1024);
     constexpr uint64_t STAGE_INC = (uint64_t)(SM::STAGE_BYTES >> 4);
-    int s = 0;
-    uint32_t ph = 0;
     for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
         int org[4], n_tile;
         tile_origin(tile, org, n_tile);
@@ -339,20 +330,20 @@ tapgemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
         int prev_s = -1;
 #pragma unroll 1
         for (int it = 0; it < total_iters; ++it) {
-            mbar_wait(&full_bar[s], ph);
-            const uint64_t da = desc_a0 + STAGE_INC * (uint64_t)s;
-            const uint64_t db = desc_b0 + STAGE_INC * (uint64_t)s;
+            ring.wait_full();
+            const uint64_t da = desc_a0 + STAGE_INC * (uint64_t)ring.s;
+            const uint64_t db = desc_b0 + STAGE_INC * (uint64_t)ring.s;
             wgmma_fence();
 #pragma unroll
             for (int k = 0; k < TG_BK / 16; ++k) tg_mma_k16<BN>(acc, da + 2 * k, db + 2 * k);
             wgmma_commit();
             wgmma_wait<1>();                         // the MMAs of the previous stage have retired: release it
-            if (prev_s >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_s]);
-            prev_s = s;
-            if (++s == NS) { s = 0; ph ^= 1; }
+            if (prev_s >= 0) ring.release(prev_s);
+            prev_s = ring.s;
+            ring.advance();
         }
         wgmma_wait<0>();
-        if (prev_s >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_s]);
+        if (prev_s >= 0) ring.release(prev_s);
 
         tg_epilogue<BN, EPI>(acc, p, org, n_tile, cw, row_in_wg, q4);
     }
