@@ -149,8 +149,10 @@ int star_upsample2x(const void* X, void* out, int BT, int H, int W, int C, int c
 /* ---- temporal VAE (video_to_video_model.py:141-161 -> diffusers AutoencoderKLTemporalDecoder) ----------------
  * The single-head (d = 512) mid-block attention runs as S = Q K^T (star_linear, N = tokens), star_softmax_rows,
  * O = S V (star_linear against V^T).  star_softmax_rows: in place over the first `cols` entries of each
- * 16-byte-aligned row of the fp16 matrix S[rows, ld] (logits already scaled), columns cols..ld-1 zeroed. */
-int star_softmax_rows(void* S, long long ld, long long rows, int cols, void* stream);
+ * 16-byte-aligned row of the fp16 matrix S[rows, ld] (logits already scaled), columns cols..ld-1 zeroed.  Each row is
+ * split over a cluster of ctas_per_row (1..8) CTAs that each stage at most 102 400 columns in shared memory, so
+ * cols <= ctas_per_row * 102400; the caller picks ctas_per_row from the row length.  ctas_per_row = 1 is one CTA per row. */
+int star_softmax_rows(void* S, long long ld, long long rows, int cols, int ctas_per_row, void* stream);
 /* decoder tail: time_conv_out = Conv3d(3,3,(3,1,1),padding (1,0,0)) over X[(b t hw), ldx] (3 valid channels) fused with
  * the tokens -> (b t, 3, h, w) layout change; W27 = weight [3][3][3] (co, ci, dt) fp16, bias3 fp16, out fp16. */
 int star_vae_head(const void* X, long long ldx, const void* W27, const void* bias3, void* out, int B, int T,

@@ -116,6 +116,30 @@ STAR_DEVINL uint8_t* dyn_smem_1024() {
 // ---------------------------------------------------------------- fences
 STAR_DEVINL void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
+// ---------------------------------------------------------------- thread-block clusters
+STAR_DEVINL uint32_t cluster_ctarank() {
+    uint32_t r;
+    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+    return r;
+}
+STAR_DEVINL uint32_t cluster_nctarank() {
+    uint32_t n;
+    asm volatile("mov.u32 %0, %%cluster_nctarank;" : "=r"(n));
+    return n;
+}
+// Every thread of every CTA of the cluster arrives (release: its earlier shared-memory writes become visible to the
+// cluster) and waits (acquire) for all of them; both must be reached by whole warps.
+STAR_DEVINL void cluster_arrive() { asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory"); }
+STAR_DEVINL void cluster_wait() { asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory"); }
+// The float at the same shared-memory offset as p in the CTA of cluster rank `rank` (distributed shared memory).
+STAR_DEVINL float ld_dsmem_f32(const float* p, uint32_t rank) {
+    uint32_t a;
+    float v;
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(a) : "r"(smem_u32(p)), "r"(rank));
+    asm volatile("ld.shared::cluster.f32 %0, [%1];" : "=f"(v) : "r"(a) : "memory");
+    return v;
+}
+
 // ---------------------------------------------------------------- TMA
 STAR_DEVINL void tma_prefetch_desc(const CUtensorMap* m) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(m)) : "memory");

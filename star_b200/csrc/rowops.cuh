@@ -884,26 +884,36 @@ __global__ void s2_split_kernel(const __half* __restrict__ x, __half* __restrict
     }
 }
 // ------------------------------------------------------------------ single-head attention pieces (VAE mid block)
-// In-place softmax over the first `cols` entries of each row of S[rows, ld] (fp16 logits, already scaled);
-// one CTA per row, the row staged in shared memory, statistics in fp32.  Columns cols..ld-1 are zeroed.
+// In-place softmax over the first `cols` entries of each row of S[rows, ld] (fp16 logits, already scaled), statistics in
+// fp32.  Columns cols..ld-1 are zeroed.  Each row is handled by one cluster of n CTAs (grid rows * n): CTA r stages columns
+// [r seg, (r + 1) seg) of the row (seg a multiple of 8; a segment may be short or empty) in its shared memory, so every
+// logit is read once and written once.  The CTAs' maxima and then their exp-sums are exchanged through distributed shared
+// memory and combined in rank order; with n = 1 both combines are exact and the kernel computes what a one-CTA-per-row
+// kernel does.
+constexpr int SOFTMAX_SEG_MAX = 102400;     // columns one CTA stages: 200 KiB of fp16
 __global__ void __launch_bounds__(256)
-softmax_rows_kernel(__half* __restrict__ S, long long ld, int cols) {
+softmax_rows_kernel(__half* __restrict__ S, long long ld, int cols, int seg) {
     extern __shared__ __align__(16) unsigned char sm_raw[];
     __half* row_s = reinterpret_cast<__half*>(sm_raw);
     __shared__ float red[8];
-    __half* row = S + (long long)blockIdx.x * ld;
-    const int tid = threadIdx.x, nv = cols / 8;
+    __shared__ float stat[2];                  // this CTA's max and exp-sum, read by the whole cluster
+    const uint32_t rank = cluster_ctarank(), n = cluster_nctarank();
+    const int c0 = (int)rank * seg;
+    const int len = max(0, min(cols - c0, seg));
+    __half* row = S + (long long)(blockIdx.x / n) * ld;
+    __half* sg = row + min(c0, cols);          // this CTA's segment
+    const int tid = threadIdx.x, nv = len / 8;
     float mx = -INFINITY;
     for (int i = tid; i < nv; i += 256) {
-        const uint4 u = reinterpret_cast<const uint4*>(row)[i];
+        const uint4 u = reinterpret_cast<const uint4*>(sg)[i];
         reinterpret_cast<uint4*>(row_s)[i] = u;
         float f[8];
         unpack8(u, f);
 #pragma unroll
         for (int j = 0; j < 8; ++j) mx = fmaxf(mx, f[j]);
     }
-    for (int i = nv * 8 + tid; i < cols; i += 256) {
-        const __half h = row[i];
+    for (int i = nv * 8 + tid; i < len; i += 256) {
+        const __half h = sg[i];
         row_s[i] = h;
         mx = fmaxf(mx, __half2float(h));
     }
@@ -913,25 +923,37 @@ softmax_rows_kernel(__half* __restrict__ S, long long ld, int cols) {
     mx = red[0];
 #pragma unroll
     for (int w = 1; w < 8; ++w) mx = fmaxf(mx, red[w]);
-    __syncthreads();
+    if (tid == 0) stat[0] = mx;
+    cluster_arrive();                          // also orders this CTA's reads of red before its rewrite below
+    cluster_wait();
+    mx = -INFINITY;
+    for (uint32_t r = 0; r < n; ++r) mx = fmaxf(mx, ld_dsmem_f32(&stat[0], r));
     float sum = 0.f;
-    for (int i = tid; i < cols; i += 256) sum += __expf(__half2float(row_s[i]) - mx);
+    for (int i = tid; i < len; i += 256) sum += __expf(__half2float(row_s[i]) - mx);
     sum = warp_sum(sum);
     if ((tid & 31) == 0) red[tid >> 5] = sum;
     __syncthreads();
     sum = 0.f;
 #pragma unroll
     for (int w = 0; w < 8; ++w) sum += red[w];
+    if (tid == 0) stat[1] = sum;
+    cluster_arrive();
+    cluster_wait();
+    sum = 0.f;
+    for (uint32_t r = 0; r < n; ++r) sum += ld_dsmem_f32(&stat[1], r);
+    cluster_arrive();                          // this CTA reads no peer's shared memory from here on
     const float inv = 1.f / sum;
     for (int i = tid; i < nv; i += 256) {
         float f[8];
         unpack8(reinterpret_cast<const uint4*>(row_s)[i], f);
 #pragma unroll
         for (int j = 0; j < 8; ++j) f[j] = __expf(f[j] - mx) * inv;
-        reinterpret_cast<uint4*>(row)[i] = pack8(f);
+        reinterpret_cast<uint4*>(sg)[i] = pack8(f);
     }
-    for (long long i = nv * 8 + tid; i < ld; i += 256)
-        row[i] = i < cols ? __float2half_rn(__expf(__half2float(row_s[i]) - mx) * inv) : __float2half_rn(0.f);
+    for (int i = nv * 8 + tid; i < len; i += 256) sg[i] = __float2half_rn(__expf(__half2float(row_s[i]) - mx) * inv);
+    if (rank + 1 == n)
+        for (long long i = cols + tid; i < ld; i += 256) row[i] = __float2half_rn(0.f);
+    cluster_wait();                            // no CTA exits while a peer may still read its stat
 }
 
 // ------------------------------------------------------------------ VAE decoder head

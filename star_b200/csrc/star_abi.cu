@@ -220,7 +220,7 @@ static int star_init_on_current(int device) {
     STAR_SMEM_ATTR(temporal_attn2_kernel<48>, TA2_WARPS * 3 * 48 * TA2_PITCH);
     STAR_SMEM_ATTR(temporal_attn2_kernel<64>, TA2_WARPS * 3 * 64 * TA2_PITCH);
     STAR_SMEM_ATTR(temporal_attn_long_kernel, TattnLongSmem::TOTAL);
-    STAR_SMEM_ATTR(softmax_rows_kernel, 200 * 1024);
+    STAR_SMEM_ATTR(softmax_rows_kernel, SOFTMAX_SEG_MAX * 2);
 #undef STAR_SMEM_ATTR
     g_sms[device] = prop.multiProcessorCount;
     return 0;
@@ -662,15 +662,31 @@ int star_upsample2x_crop(const void* X, void* out, int BT, int H, int W, int C, 
     return star_upsample2x(X, out, BT, H, W, C, 1, stream);
 }
 
-int star_softmax_rows(void* S, long long ld, long long rows, int cols, void* stream) {
+int star_softmax_rows(void* S, long long ld, long long rows, int cols, int ctas_per_row, void* stream) {
     STAR_CHECK_INIT();
     if (rows <= 0) return 0;
     if (ld % 8 || reinterpret_cast<uintptr_t>(S) % 16) return fail("star_softmax_rows: rows must be 16-byte aligned (ld %% 8 == 0)");
     if (cols <= 0 || cols > ld) return fail("star_softmax_rows: need 0 < cols <= ld");
-    const size_t smem = ((size_t)cols * 2 + 15) / 16 * 16;
-    if (smem > 200 * 1024) return fail("star_softmax_rows: %d columns do not fit in shared memory", cols);
-    if (rows > 0x7fffffffll) return fail("star_softmax_rows: too many rows");
-    softmax_rows_kernel<<<(unsigned)rows, 256, smem, (cudaStream_t)stream>>>((__half*)S, ld, cols);
+    if (ctas_per_row < 1 || ctas_per_row > 8) return fail("star_softmax_rows: ctas_per_row=%d outside [1, 8], the portable cluster size", ctas_per_row);
+    if (cols > ctas_per_row * SOFTMAX_SEG_MAX)
+        return fail("star_softmax_rows: %d columns do not fit in shared memory (%d CTAs of %d columns per row)", cols,
+                    ctas_per_row, SOFTMAX_SEG_MAX);
+    if (rows * ctas_per_row > 0x7fffffffll) return fail("star_softmax_rows: too many rows");
+    // segments of a multiple of 8 columns keep every CTA's 128-bit loads aligned, and stay <= SOFTMAX_SEG_MAX (one too)
+    const int seg = ((cols + ctas_per_row - 1) / ctas_per_row + 7) / 8 * 8;
+    cudaLaunchConfig_t cfg = {};
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = (unsigned)ctas_per_row;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    cfg.gridDim = dim3((unsigned)(rows * ctas_per_row));
+    cfg.blockDim = dim3(256);
+    cfg.dynamicSmemBytes = (size_t)seg * 2;
+    cfg.stream = (cudaStream_t)stream;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    STAR_CUDA(cudaLaunchKernelEx(&cfg, softmax_rows_kernel, (__half*)S, ld, cols, seg));
     STAR_LAUNCH_CHECK("softmax_rows");
     return 0;
 }

@@ -43,7 +43,7 @@ SIGNATURES = {
     "star_time_avgpool2": (_i, [_p, _p, _i, _ll, _i, _p]),
     "star_upsample2x_crop": (_i, [_p, _p, _i, _i, _i, _i, _p]),
     "star_upsample2x": (_i, [_p, _p, _i, _i, _i, _i, _i, _p]),
-    "star_softmax_rows": (_i, [_p, _ll, _ll, _i, _p]),
+    "star_softmax_rows": (_i, [_p, _ll, _ll, _i, _i, _p]),
     "star_vae_head": (_i, [_p, _ll, _p, _p, _p, _i, _i, _ll, _p]),
     "star_conv2d_s2p_workspace_bytes": (_ll, [_i, _i, _i, _i, _i, _i, _i, _i]),
     "star_conv2d_3x3_s2p": (_i, [_p, _p, _p, _p, _ll, _p, _i, _i, _i, _i, _i, _i, _i, _i, _i, _p]),

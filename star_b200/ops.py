@@ -365,11 +365,12 @@ def upsample2x(x, BT, H, W, out=None):
 
 
 @_traced
-def softmax_rows(s, cols):
-    """in-place row softmax of the fp16 matrix s[rows, ld] over its first `cols` columns"""
+def softmax_rows(s, cols, ctas_per_row=1):
+    """in-place row softmax of the fp16 matrix s[rows, ld] over its first `cols` columns; each row is split over a cluster
+    of ctas_per_row CTAs (1..8) of at most 102 400 columns each"""
     L, _ = _bind(s)
     ld = _rowmajor(s, "s")
-    _L.check(L, L.star_softmax_rows(_p(s), ld, s.shape[0], int(cols), _st()), "star_softmax_rows")
+    _L.check(L, L.star_softmax_rows(_p(s), ld, s.shape[0], int(cols), int(ctas_per_row), _st()), "star_softmax_rows")
     return s
 
 

@@ -273,8 +273,11 @@ class AutoencoderKLTemporalDecoder(nn.Module):
         q = ops.linear(xn, a["q"][0], a["q"][1])
         k = ops.linear(xn, a["k"][0], a["k"][1])
         ld = (HW + 7) // 8 * 8
-        # logits are materialised for a block of query rows at a time (<= 0.6 GB at any resolution the softmax kernel accepts:
-        # 102 400 key columns = a 2 560 x 2 560-pixel frame); columns HW..ld of S are zeroed by star_softmax_rows
+        # a row of logits is spread over as many CTAs as its keys need (one CTA stages <= 102 400 of them, a 2 560 x 2 560-pixel
+        # frame; 234 576 at 720p -> 4x take 3).  Rows that fit one CTA make the default call, which is also the signature of
+        # the emulated kernel in oracle/kernel_ref.py.  Logits are materialised for a block of query rows at a time (<= 0.6 GB
+        # up to 819 200 key columns, the most 8 CTAs hold); columns HW..ld of S are zeroed by star_softmax_rows
+        cluster = {} if HW <= 102400 else {"ctas_per_row": -(-HW // 102400)}
         rb = max(128, min(HW, (1 << 28) // ld // 128 * 128))
         S = torch.empty((min(rb, HW), ld), dtype=HALF, device=x.device)
         vt = torch.zeros((C, ld), dtype=HALF, device=x.device)
@@ -286,7 +289,7 @@ class AutoencoderKLTemporalDecoder(nn.Module):
                 r1 = min(HW, r0 + rb)
                 Sb = S[: r1 - r0]
                 ops.linear(q[f * HW + r0:f * HW + r1], k[rows], out=Sb[:, :HW])   # logits, 1/sqrt(C) already in W_q
-                ops.softmax_rows(Sb, HW)
+                ops.softmax_rows(Sb, HW, **cluster)
                 ops.linear(Sb, vt, out=o[f * HW + r0:f * HW + r1])          # P V
         return ops.linear(o, a["o"][0], a["o"][1], residual=x)
 

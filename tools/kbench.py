@@ -154,6 +154,20 @@ def bench_tattn():
         del qkv
 
 
+def bench_softmax():
+    """Row softmax of the temporal VAE's mid-block attention: rows of one frame's logits, a row spread over a cluster of
+    ceil(cols / 102 400) CTAs.  234 576 columns = a 720p -> 4x frame (362x648 latent), 528 528 = 1080p -> 4x (542x976).
+    Bytes = the logits read once and written once (2 x rows x ld x 2 B)."""
+    for cols in (26352, 102400, 234576, 528528):
+        ld = (cols + 7) // 8 * 8
+        rows = max(128, (1 << 28) // ld // 128 * 128)                   # temporal_vae._attention's row block
+        n = -(-cols // 102400)
+        s = rnd(rows, ld, scale=3.0)
+        report(f"softmax_rows {rows}x{cols}, {n} CTA(s) per row", timeit(lambda: O.softmax_rows(s, cols, n), 20),
+               bytes_=2.0 * rows * ld * 2)
+        del s
+
+
 def card():
     import subprocess
     try:

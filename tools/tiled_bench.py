@@ -9,9 +9,11 @@ torch.cuda.max_memory_allocated, untiled and with tiles of 90x160 latent pixels 
                                   fits in 80 % of the free memory (otherwise skipped, not measured)
   362x648 (720p -> 4x),   F = 32: tiled only
 
-and the pixel legs of a 720p -> 4x clip (2880x5120): peak memory of one frame's bilinear upsample + VAE encode and of one
-3-frame VAE decode window (untiled VAE, synthetic weights), then enhance_frames(tile_size=(90, 160)) end to end on an
-8-frame 720p clip with one solver step (skipped when a pixel leg fails; the failure is printed).  python tools/tiled_bench.py [--frames 32] [--skip-e2e]"""
+and the pixel legs of a 720p -> 4x clip (2880x5120): time and peak memory of one frame's bilinear upsample + VAE encode and
+of one 3-frame VAE decode window (untiled VAE, synthetic weights), each with the share of its op time spent in the VAE's
+mid-block attention (a second, traced run), then enhance_frames(tile_size=(90, 160)) end to end on an 8-frame 720p clip with
+one solver step (skipped when a pixel leg fails; the failure is printed).
+python tools/tiled_bench.py [--frames 32] [--skip-e2e | --skip-latent]"""
 import argparse
 import os
 import sys
@@ -122,32 +124,69 @@ def synth_vae(dev):
     return vae.eval().requires_grad_(False)
 
 
+def timed(fn, dev):
+    """fn()'s result, its time (CUDA events) and the peak memory allocated while it ran"""
+    torch.cuda.synchronize()
+    torch.cuda.empty_cache()
+    torch.cuda.reset_peak_memory_stats(dev)
+    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    a.record()
+    out = fn()
+    b.record()
+    torch.cuda.synchronize()
+    return out, a.elapsed_time(b), torch.cuda.max_memory_allocated(dev)
+
+
+def attention_share(fn):
+    """fn() traced op by op (ops.trace_begin / trace_end): (ms in the VAE's mid-block attention, ms in all ops)"""
+    from star_b200 import ops
+    from star_b200.video_to_video.modules.temporal_vae import AutoencoderKLTemporalDecoder as AE
+    spans, orig = [], AE.__dict__["_attention"]
+
+    def attention(a, x, n, HW):
+        i0 = len(ops._trace)
+        out = orig.__func__(a, x, n, HW)
+        spans.append((i0, len(ops._trace)))
+        return out
+    AE._attention = staticmethod(attention)
+    try:
+        ops.trace_begin()
+        fn()
+        rec = ops.trace_end()
+    finally:
+        AE._attention = orig
+    return sum(ms for i0, i1 in spans for _, _, ms in rec[i0:i1]), sum(ms for _, _, ms in rec)
+
+
 def pixel_legs(pipe, dev, lr=(720, 1280), scale=4):
     from star_b200.video_to_video.video_to_video_model import pad_to_fit
     th, tw = lr[0] * scale, lr[1] * scale
     pad = pad_to_fit(th, tw)
     base = torch.cuda.memory_allocated(dev)
     frame = torch.rand(1, 3, *lr, device=dev) * 2 - 1
-    torch.cuda.synchronize()
-    torch.cuda.reset_peak_memory_stats(dev)
+    encode = lambda: pipe.vae_encode(pipe.upsample_pad(frame, th, tw, pad).unsqueeze(0))   # noqa: E731  (no autocast, as _test_on_device)
     try:
-        z = pipe.vae_encode(pipe.upsample_pad(frame, th, tw, pad).unsqueeze(0))         # as _test_on_device: no autocast
-        torch.cuda.synchronize()
-        print(f"pixel {th}x{tw}: one frame bilinear x{scale} + VAE encode peak {torch.cuda.max_memory_allocated(dev) / GB:6.1f} GiB "
-              f"(VAE weights and model resident {base / GB:.1f} GiB), latent {tuple(z.shape)}", flush=True)
+        z, ms, peak = timed(encode, dev)
+        att, tot = attention_share(encode)
+        print(f"pixel {th}x{tw}: one frame bilinear x{scale} + VAE encode {ms / 1e3:.2f} s, peak {peak / GB:6.1f} GiB "
+              f"(VAE weights and model resident {base / GB:.1f} GiB), latent {tuple(z.shape)}; traced: mid-block attention "
+              f"{att / 1e3:.2f} of {tot / 1e3:.2f} s of op time ({100 * att / tot:.1f} %)", flush=True)
+        del z
     except (torch.cuda.OutOfMemoryError, StarError) as e:
         print(f"pixel {th}x{tw}: one frame upsample + encode failed: {e}", flush=True)
         return False
     zl = torch.randn(1, 4, 3, (th + pad[2] + pad[3]) // 8, (tw + pad[0] + pad[1]) // 8, device=dev)
-    torch.cuda.empty_cache()
-    torch.cuda.reset_peak_memory_stats(dev)
-    try:
+
+    def decode():
         with torch.autocast("cuda"):
-            out = pipe.vae_decode_chunk(zl, chunk_size=3)
-        torch.cuda.synchronize()
-        print(f"pixel {th}x{tw}: one 3-frame VAE decode window peak {torch.cuda.max_memory_allocated(dev) / GB:6.1f} GiB, "
-              f"output {tuple(out.shape)}", flush=True)
+            return pipe.vae_decode_chunk(zl, chunk_size=3)
+    try:
+        out, ms, peak = timed(decode, dev)
+        shape = tuple(out.shape)
         del out
+        att, tot = attention_share(decode)
+        print(f"pixel {th}x{tw}: one 3-frame VAE decode window {ms / 1e3:.2f} s, peak {peak / GB:6.1f} GiB, output {shape}; "
+              f"traced: mid-block attention {att / 1e3:.2f} of {tot / 1e3:.2f} s of op time ({100 * att / tot:.1f} %)", flush=True)
     except (torch.cuda.OutOfMemoryError, StarError) as e:
         print(f"pixel {th}x{tw}: one 3-frame decode window failed: {e}", flush=True)
         return False
@@ -177,6 +216,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--frames", type=int, default=32)
     ap.add_argument("--skip-e2e", action="store_true", help="latent legs only")
+    ap.add_argument("--skip-latent", action="store_true", help="pixel legs and enhance_frames only")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("tiled_bench needs a CUDA device")
@@ -189,7 +229,8 @@ def main():
     pipe = VideoToVideo_sr(SimpleNamespace(model_path=None), device=dev, text_encoder=lambda s: ny, vae=object(), generator=net)
     print(f"# full ControlledV2VUNet, synthetic fp16 weights {torch.cuda.memory_allocated(dev) / GB:.2f} GiB; one solver step "
           "per line", flush=True)
-    latent_legs(pipe, net, args.frames, dev)
+    if not args.skip_latent:
+        latent_legs(pipe, net, args.frames, dev)
     if not args.skip_e2e:
         pipe.vae = synth_vae(dev)
         if pixel_legs(pipe, dev):
