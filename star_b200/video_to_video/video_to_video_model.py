@@ -12,6 +12,8 @@ Mirrors ``VideoToVideo_sr`` of the reference's video_to_video/video_to_video_mod
 * the text encoder (open_clip) is an un-vendored third-party package: it is imported lazily, and
   ready-made objects can be injected (``text_encoder=``, ``vae=``, ``generator=``), which is how the
   tests and the benchmark run on boxes without those packages or checkpoints;
+* the LR frames are uploaded, upsampled and encoded one at a time, and ``enhance_frames_iter`` yields the finished frames one
+  3-frame decode window at a time, so in a single process the device memory of a clip grows only by its latents;
 * with ``torch.distributed`` initialised (one process per GPU) the whole entry is sharded (SURVEY 8e):
   - each rank uploads, upsamples and VAE-encodes only its contiguous share of the frames; the latents (0.42 MB per
     frame) are all-gathered, so every rank conditions on the SAME posterior sample (the reference draws it once);
@@ -160,43 +162,129 @@ class VideoToVideo_sr():
                        max_chunk_len=32, uint8=True, tile_size=None, tile_overlap=16):
         """test() + the CLI's post-processing (inference_sr.py:77-80: tensor2vid, adain_color_fix against the LR clip) with the
         post-processing on the GPU: returns (F, H, W, 3) frames in [0, 255] on the CPU -- uint8 by default, i.e. a quarter of the
-        device->host traffic of test()'s fp32 tensor."""
+        device->host traffic of test()'s fp32 tensor.  In a single process the frames come from enhance_frames_iter, so the
+        device holds no whole-clip tensor at output resolution."""
+        if _dist_info()[0] == 1:
+            (h, w) = input['target_res']
+            out = torch.empty((input['video_data'].shape[0], h, w, 3), dtype=torch.uint8 if uint8 else torch.float32)
+            for s, frames in self.enhance_frames_iter(input, total_noise_levels, steps, solver_mode, guide_scale, max_chunk_len,
+                                                      uint8, tile_size, tile_overlap):
+                out[s:s + frames.shape[0]] = frames
+            return out
         vid = self._test_on_device(input, total_noise_levels, steps, solver_mode, guide_scale, max_chunk_len,
                                    tile_size, tile_overlap).float()
         if vid.is_cuda:
             return ops.adain_color_fix(vid, input['video_data'].to(vid.device).float(), uint8=uint8).cpu()
         raise NotImplementedError("enhance_frames runs the GPU post-processing kernels; use test() + the reference's CPU helpers otherwise")
 
-    def _test_on_device(self, input, total_noise_levels, steps, solver_mode, guide_scale, max_chunk_len, tile_size=None,
-                        tile_overlap=16):
+    def enhance_frames_iter(self, input: Dict[str, Any], total_noise_levels=1000, steps=50, solver_mode='fast', guide_scale=7.5,
+                            max_chunk_len=32, uint8=True, tile_size=None, tile_overlap=16):
+        """enhance_frames as a generator of (start, frames) in clip order, one 3-frame VAE decode window at a time: frames
+        (k, H, W, 3) of the clip's frames [start, start + k) on the CPU (pinned), uint8 or fp32 in [0, 255], owned by the caller.
+
+        The LR frames are encoded one at a time and the denoised latent is decoded, cropped and colour-corrected one window at
+        a time, so the device memory a clip needs grows only by its fp32 latents (0.42 MB per frame each at 240p -> 960p).  The frames
+        equal enhance_frames' byte for byte.  The next window is decoded on the GPU while the caller handles the current one.
+        Single process only: under a process group of more than one rank use enhance_frames."""
+        if _dist_info()[0] > 1:
+            raise NotImplementedError("enhance_frames_iter runs in a single process; under torch.distributed with more than one "
+                                      "rank use enhance_frames, which shards the decode across the ranks")
+        if torch.device(self.device).type != 'cuda':
+            raise NotImplementedError("enhance_frames_iter runs the GPU post-processing kernels; use test() + the reference's "
+                                      "CPU helpers otherwise")
+        return self._enhanced_windows(input, total_noise_levels, steps, solver_mode, guide_scale, max_chunk_len, uint8,
+                                      tile_size, tile_overlap)
+
+    @torch.no_grad()
+    def _enhanced_windows(self, input, total_noise_levels, steps, solver_mode, guide_scale, max_chunk_len, uint8, tile_size,
+                          tile_overlap, chunk_size=3):
         video_data = input['video_data']
-        y = input['y']
+        (h, w) = input['target_res']
+        gen_vid, (w1, _, h1, _) = self._sample_latents(input, total_noise_levels, steps, solver_mode, guide_scale, max_chunk_len,
+                                                       tile_size, tile_overlap)
+        z = rearrange(gen_vid, "b c f h w -> (b f) c h w")
+        n = z.shape[0]
+        stream = torch.cuda.current_stream(self.device)
+
+        def launch(s):
+            """enqueue window [s, s + k): LR upload, decode (the windows and autocast of _test_on_device), crop, colour fix,
+            copy into a fresh pinned host tensor; returns (s, host tensor, device result, its copy's event)"""
+            k = min(chunk_size, n - s)
+            lr = self._upload_lr(video_data[s:s + k]).float()
+            with torch.autocast('cuda'):
+                dec = self.temporal_vae_decode(z[s:s + k], k)
+            vid = dec[:, :, h1:h + h1, w1:w + w1].permute(1, 0, 2, 3).unsqueeze(0).float()
+            out = ops.adain_color_fix(vid, lr, uint8=uint8)
+            host = torch.empty(out.shape, dtype=out.dtype, pin_memory=True)
+            host.copy_(out, non_blocking=True)
+            done = torch.cuda.Event()
+            done.record(stream)
+            return s, host, out, done
+
+        pending = launch(0) if n else None
+        try:
+            while pending is not None:
+                s, host, staged, done = pending
+                pending = launch(s + chunk_size) if s + chunk_size < n else None
+                done.synchronize()
+                del staged                     # held until its copy to `host` has completed
+                yield s, host
+        finally:
+            stream.synchronize()              # a caller that stops early leaves no work in flight
+
+    def _upload_lr(self, frames):
+        """LR frames -> self.device.  A host tensor goes through pinned memory so that the copy is queued behind the work
+        already on the stream instead of waiting for it on the host."""
+        if frames.device.type == 'cpu' and torch.device(self.device).type == 'cuda':
+            frames = frames.pin_memory()
+        return frames.to(self.device, non_blocking=True)
+
+    def _encode_frames(self, frames, target_h, target_w, padding):
+        """LR frames (n, 3, h, w) -> their VAE latent (1, 4, n, H/8, W/8) on self.device, one frame at a time: upload,
+        upsample_pad, vae_encode (posterior sample times the scaling factor), written into the clip's latent.  Only one
+        canvas-sized frame exists at a time.  vae_encode draws one posterior sample per frame, like the reference (ref :141-161),
+        so the random draws and the latent are those of encoding the whole upsampled clip."""
+        n = frames.shape[0]
+        feat = None
+        for i in range(n):
+            z = self.vae_encode(self.upsample_pad(self._upload_lr(frames[i:i + 1]), target_h, target_w, padding).unsqueeze(0))
+            if feat is None:
+                feat = z.new_empty((1, z.shape[1], n, *z.shape[3:]))
+            feat[:, :, i:i + 1] = z
+        if feat is None:
+            w1, w2, h1, h2 = padding
+            feat = torch.zeros((1, 4, 0, (target_h + h1 + h2) // 8, (target_w + w1 + w2) // 8), device=self.device)
+        return feat
+
+    def _sample_latents(self, input, total_noise_levels, steps, solver_mode, guide_scale, max_chunk_len, tile_size=None,
+                        tile_overlap=16):
+        """encode (this rank's share of the frames, latents all-gathered) + denoise_latents: (denoised latent, padding)"""
+        video_data = input['video_data']
         (target_h, target_w) = input['target_res']
         world, rank = _dist_info()
         frames_num = video_data.shape[0]
         bounds = _shard_bounds(frames_num, world)
         lo, hi = bounds[rank]
-        # this rank's frames only: upload (LR frames), bilinear x4 + pad-with-1 on the GPU, encode frame by frame
         padding = pad_to_fit(target_h, target_w)
-        h, w = target_h, target_w
-        local = video_data[lo:hi].to(self.device)
-        logger.info(f'video_data shape: {(frames_num, video_data.shape[1], h, w)}')
-        bs = 1
-        if hi > lo:
-            local = self.upsample_pad(local, target_h, target_w, padding)
-            feat_local = self.vae_encode(local.unsqueeze(0))
-        else:
-            lh = (h + padding[2] + padding[3]) // 8
-            lw = (w + padding[0] + padding[1]) // 8
-            feat_local = torch.zeros((1, 4, 0, lh, lw), device=self.device)
-        del local
+        logger.info(f'video_data shape: {(frames_num, video_data.shape[1], target_h, target_w)}')
+        feat_local = self._encode_frames(video_data[lo:hi], target_h, target_w, padding)
         video_data_feature = feat_local if world == 1 else \
             _all_gather_varlen(feat_local.float(), [b - a for a, b in bounds], 2)
-        y = self._encode_text(y)
+        del feat_local
+        y = self._encode_text(input['y'])
         tiles = {} if tile_size is None else {'tile_size': tile_size, 'tile_overlap': tile_overlap}
         gen_vid = self.denoise_latents(video_data_feature, y, None, total_noise_levels, steps, solver_mode,
                                        guide_scale, max_chunk_len, **tiles)
         logger.info('sampling, finished.')
+        return gen_vid, padding
+
+    def _test_on_device(self, input, total_noise_levels, steps, solver_mode, guide_scale, max_chunk_len, tile_size=None,
+                        tile_overlap=16):
+        (h, w) = input['target_res']
+        bs = 1
+        gen_vid, padding = self._sample_latents(input, total_noise_levels, steps, solver_mode, guide_scale, max_chunk_len,
+                                                tile_size, tile_overlap)
+        world, _ = _dist_info()
         w1, w2, h1, h2 = padding
         with torch.autocast('cuda', enabled=torch.cuda.is_available()):
             if world == 1:
