@@ -4,9 +4,10 @@
 // replaces xformers.ops.memory_efficient_attention at unet_v2v.py:179/:184 for the
 // spatial self-attention (N = H*W up to 26 352) and the text cross-attention (Nk = 77).
 //
-// One CTA = 128 query rows of one (batch, head).  Warp roles (384 threads):
-//   warpgroup 0      one TMA producer thread: Q once, then K/V tiles (128 keys) through a ring of stages
-//   warpgroups 1, 2  64 query rows each, one attn_block_step<128> per K/V tile
+// One CTA = 192 query rows of one (batch, head).  Warp roles (512 threads):
+//   warpgroup 0        one TMA producer thread: Q once, then K/V tiles (128 keys) through a ring of stages
+//   warpgroups 1 - 3   64 query rows each, one attn_block_step<128> per K/V tile: a third consumer gives the scheduler
+//                      a third independent chain of MMA, MUFU and FMA work to interleave
 // Keys beyond Nk are zero-filled by TMA and masked; with `causal` the key tiles past the last query row are skipped.
 // attn_block_step is also the consumer step of temporal_attn_long_kernel (tattn_long.cuh).
 #pragma once
@@ -15,12 +16,12 @@
 
 namespace star {
 
-constexpr int AT_BQ = 128;
+constexpr int AT_BQ = 192;
 constexpr int AT_BKV = 128;
 constexpr int AT_D = 64;
 constexpr int AT_KV_STAGES = 4;
-constexpr int AT_THREADS = 384;
-constexpr int AT_CONSUMER_WARPS = 8;
+constexpr int AT_THREADS = 512;
+constexpr int AT_CONSUMER_WARPS = 12;
 
 struct AttnParams {
     int Nq, Nk;
@@ -32,9 +33,10 @@ struct AttnParams {
 };
 
 struct AttnSmem {
-    static constexpr int TILE = AT_BQ * AT_D * 2;             // 16 KB (Q, and one K or V tile of 128 keys)
+    static constexpr int Q_TILE = AT_BQ * AT_D * 2;           // 24 KB
+    static constexpr int TILE = AT_BKV * AT_D * 2;            // 16 KB: one K or V tile
     static constexpr int OFF_Q = 0;
-    static constexpr int OFF_K = OFF_Q + TILE;
+    static constexpr int OFF_K = OFF_Q + Q_TILE;
     static constexpr int OFF_V = OFF_K + AT_KV_STAGES * TILE;
     static constexpr int OFF_BAR = OFF_V + AT_KV_STAGES * TILE;
     static constexpr int TOTAL = OFF_BAR + 256 + 1024;
@@ -122,7 +124,9 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
     uint64_t* q_full = reinterpret_cast<uint64_t*>(smem + AttnSmem::OFF_BAR);
     StageRing<AT_KV_STAGES> kv(q_full + 1);
 
-    const int wg = threadIdx.x >> 7;
+    // warp-uniform through the shuffle, so the Q descriptor of the warpgroup lives in uniform registers: held in vector
+    // registers, dq + 2k spills at the 512-thread register budget
+    const int wg = __shfl_sync(0xffffffffu, threadIdx.x >> 7, 0);
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
     const int q0 = blockIdx.x * AT_BQ;
@@ -145,7 +149,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
     if (wg == 0) {
         asm volatile("setmaxnreg.dec.sync.aligned.u32 24;");
         if (threadIdx.x == 0) {
-            mbar_expect_tx(q_full, AttnSmem::TILE);
+            mbar_expect_tx(q_full, AttnSmem::Q_TILE);
             tma_load_3d(smem + AttnSmem::OFF_Q, &tmap_q, q_full, head * AT_D, q0, batch);
             for (int j = 0; j < nt; ++j) {
                 kv.wait_empty();
@@ -159,7 +163,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
         return;
     }
 
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 240;");
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 160;");         // 128 x 24 + 384 x 160 <= 64K registers
     const int cw = wg - 1;
     const int q4 = lane & 3;
     const int row_in_wg = (warp & 3) * 16 + (lane >> 2);
@@ -192,8 +196,10 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constan
         l += __shfl_xor_sync(0xffffffffu, l, 1);
         l += __shfl_xor_sync(0xffffffffu, l, 2);
         const float inv = 1.0f / l;
-        if (qrow[h] < p.Nq) {
-            __half* op = p.out + ((long long)batch * p.Nq + qrow[h]) * p.ldo + head * AT_D + 2 * q4;
+        // the row again from threadIdx, not qrow[h]: held across the key loop, qrow spills at 512 threads
+        const int row = q0 + ((int)(threadIdx.x >> 7) - 1) * 64 + row_in_wg + 8 * h;
+        if (row < p.Nq) {
+            __half* op = p.out + ((long long)batch * p.Nq + row) * p.ldo + head * AT_D + 2 * q4;
 #pragma unroll
             for (int jj = 0; jj < 8; ++jj)
                 *reinterpret_cast<uint32_t*>(op + 8 * jj) = pack_half2(o[4 * jj + 2 * h] * inv, o[4 * jj + 2 * h + 1] * inv);

@@ -393,16 +393,17 @@ static int attention_impl(const void* Q, long long ldq, const void* K, long long
     if (kv_batch_div < 1) kv_batch_div = 1;
     const int kv_batches = (batch + kv_batch_div - 1) / kv_batch_div;
     CUtensorMap tq, tk, tv;
-    unsigned box[3] = {AT_D, AT_BQ, 1};
     {
         unsigned long long dims[3] = {(unsigned long long)heads * AT_D, (unsigned long long)Nq, (unsigned long long)batch};
         unsigned long long str[3] = {1, (unsigned long long)ldq, (unsigned long long)ldq * Nq};
+        unsigned box[3] = {AT_D, AT_BQ, 1};
         if (make_tmap(&tq, Q, 3, dims, str, box)) return 1;
     }
     {
         unsigned long long dims[3] = {(unsigned long long)heads * AT_D, (unsigned long long)Nk, (unsigned long long)kv_batches};
         unsigned long long strk[3] = {1, (unsigned long long)ldk, (unsigned long long)ldk * Nk};
         unsigned long long strv[3] = {1, (unsigned long long)ldv, (unsigned long long)ldv * Nk};
+        unsigned box[3] = {AT_D, AT_BKV, 1};
         if (make_tmap(&tk, K, 3, dims, strk, box)) return 1;
         if (make_tmap(&tv, V, 3, dims, strv, box)) return 1;
     }
