@@ -48,10 +48,12 @@ int star_linear_ex(const void* A, long long lda, const void* W, const void* bias
                    long long ldo, long long rows, int K, int N, int flags, void* stream);
 
 /* Conv2d 3x3 stride 1 pad 1 on X[BT,H,W,Cin]; W9 = weight permuted to [Cout][3][3][Cin]; rowvec = per-clip time
- * embedding added before the next GroupNorm; replaces cuDNN at unet_v2v.py:612,:639,:553-554,:1552. */
+ * embedding added before the next GroupNorm; replaces cuDNN at unet_v2v.py:612,:639,:553-554,:1552.  Only output rows
+ * [row0, row0 + H_out) are computed, out = [BT, H_out, W, Cout]: a band of X whose halo rows come from X itself (the temporal
+ * VAE upsamples and convolves a large frame band by band).  row0 = 0, H_out = H is the whole frame. */
 int star_conv2d_3x3(const void* X, const void* W9, const void* bias, const void* rowvec, long long rowvec_div, long long ldrowvec,
                     const void* residual, long long ldres, void* out, long long ldo, int BT, int H, int W, int Cin,
-                    int Cout, void* stream);
+                    int Cout, int row0, int H_out, void* stream);
 /* Downsample: Conv2d 3x3 stride 2 padding (2,1) (unet_v2v.py:709-729).  Ho = (H+1)/2 + 1, Wo = (W-1)/2 + 1.
  * planes_ws: scratch of star_conv2d_s2_workspace_bytes(). */
 long long star_conv2d_s2_workspace_bytes(int BT, int H, int W, int Cin);
@@ -65,9 +67,11 @@ int star_conv2d_3x3_s2p(const void* X, const void* W9, const void* bias, void* o
                         int BT, int H, int W, int Cin, int Cout, int pad_t, int pad_b, int pad_l, int pad_r,
                         void* stream);
 /* Conv3d (3,1,1) pad (1,0,0) over frames on X[B,T,HW,Cin]; W3 = weight permuted to [Cout][3][Cin]
- * (unet_v2v.py:1209-1220). */
+ * (unet_v2v.py:1209-1220).  Runs over pixels [p0, p0 + band) of every frame: X holds that band compactly ([B, T, band, Cin]),
+ * residual and out are the full [B, T, HW] row space of which only the band's rows are read / written (the temporal VAE
+ * decodes large frames band by band).  p0 = 0, band = HW is the whole clip. */
 int star_conv_t3(const void* X, const void* W3, const void* bias, const void* residual, long long ldres, void* out,
-                 long long ldo, int B, int T, long long HW, int Cin, int Cout, void* stream);
+                 long long ldo, int B, int T, long long HW, long long p0, long long band, int Cin, int Cout, void* stream);
 /* Stem convs with Cin = 4 (unet_v2v.py:1353 input conv, :2128 input_hint_block); W9 as above.  Runs as im2col
  * (K = 36 padded to 64) + tensor-core GEMM; ws = scratch of star_conv2d_c4_workspace_bytes(). */
 long long star_conv2d_c4_workspace_bytes(int BT, int H, int W, int Cout);
@@ -100,9 +104,17 @@ int star_temporal_attention(const void* QKV, long long ld, void* O, long long ld
 int star_conv3d_causal(const void* X, const void* W27, const void* bias, const void* residual, long long ldres, void* out,
                        long long ldo, int T, int H, int W, int Cin, int Cout, void* stream);
 
+/* phases: STAR_GN_STATS computes the statistics into the workspace (star_groupnorm_workspace_bytes(nsamples, C)),
+ * STAR_GN_APPLY normalises with the workspace's statistics: each sample is viewed as frames of frame_rows rows, and rows
+ * [p0, p0 + band) of every frame are written compactly to out ([frames * band, C]), so clip statistics can be applied a pixel
+ * band at a time.  Both phases over whole samples (frame_rows = band = rows_per_sample, p0 = 0) is one GroupNorm; out may
+ * then alias X.  Split phases and bands need C <= 2048. */
+#define STAR_GN_STATS 1
+#define STAR_GN_APPLY 2
 long long star_groupnorm_workspace_bytes(int nsamples, int C);
-int star_groupnorm(const void* X, const void* gamma, const void* beta, void* out, int nsamples,
-                   long long rows_per_sample, int C, float eps, int silu, void* workspace, void* stream);
+int star_groupnorm(const void* X, const void* gamma, const void* beta, void* out, int nsamples, long long rows_per_sample, int C,
+                   float eps, int silu, long long frame_rows, long long p0, long long band, int phases, void* workspace,
+                   void* stream);
 /* SpatialNorm3D.forward of the CogVideoX 3-D VAE decoder (cp_enc_dec.py:491-510): out = GroupNorm32(X) * Ymod[src] + Bmod[src]
  * (+ SiLU, the `nonlinearity` that always follows, :673,:687,:977) over one clip of T x H x W rows.  Ymod / Bmod are conv_y(zq) /
  * conv_b(zq) evaluated at the latent's resolution (Tl, Hl, Wl): 1x1x1 convolutions commute with the nearest-neighbour

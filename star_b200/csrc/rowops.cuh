@@ -365,6 +365,33 @@ gn_apply2_kernel(const __half* __restrict__ x, const float* __restrict__ ab, __h
     }
 }
 
+// apply over a pixel band: x holds frames of frame_rows rows (frames_per_sample of them share one sample's (a, b)); rows
+// [p0, p0 + band) of every frame go compactly to out [frames * band, C].  Same per-element arithmetic as gn_apply2_kernel.
+__global__ void gn_apply_band_kernel(const __half* __restrict__ x, const float* __restrict__ ab, __half* __restrict__ out,
+                                     long long frames_per_sample, long long frame_rows, long long p0, long long band,
+                                     long long frames, int C, int silu) {
+    const int O = C / 8;
+    const long long n = frames * band * O;
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+        const long long orow = i / O;
+        const int oc = (int)(i % O);
+        const long long f = orow / band;
+        const long long sample = f / frames_per_sample;
+        float f8[8];
+        unpack8(__ldg(reinterpret_cast<const uint4*>(x + (f * frame_rows + p0 + orow % band) * C + oc * 8)), f8);
+        const float4* abp = reinterpret_cast<const float4*>(ab + (sample * C + oc * 8) * 2);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const float4 q = __ldg(abp + j);
+            float y0 = fmaf(f8[2 * j], q.x, q.y), y1 = fmaf(f8[2 * j + 1], q.z, q.w);
+            if (silu) { y0 = silu_f(y0); y1 = silu_f(y1); }
+            f8[2 * j] = y0;
+            f8[2 * j + 1] = y1;
+        }
+        reinterpret_cast<uint4*>(out)[i] = pack8(f8);
+    }
+}
+
 // GroupNorm apply of the CogVideoX 3-D VAE's SpatialNorm3D (cp_enc_dec.py:451-510): y = GN(x) * Y[src] + B[src] (+ SiLU), where
 // Y = conv_y(zq), B = conv_b(zq) are 1x1x1 convolutions of the latent and therefore commute with the nearest-neighbour
 // interpolation of zq to the feature size: they are evaluated ONCE at latent resolution (Tl, Hl, Wl) and gathered per row.

@@ -131,11 +131,14 @@ int launch_tapgemm(TapGemmParams& p, const void* A, unsigned long long lda, unsi
     long long m_tiles = 1;
     p.box_rows = 1;
     for (int i = 0; i < 4; ++i) {
+        if (p.row_ext[i] == 0) p.row_ext[i] = p.on[i];
         p.tiles[i] = (p.on[i] + p.box[i] - 1) / p.box[i];
         m_tiles *= p.tiles[i];
         p.box_rows *= p.box[i];
     }
     if (p.box_rows > TG_BM) return fail("tapgemm: box has %d rows (> %d)", p.box_rows, TG_BM);
+    for (int i = 0; i < 4; ++i)
+        if (p.rowvec && p.row_ext[i] != p.on[i]) return fail("tapgemm: rowvec rows are not defined over extended row extents");
     p.k_chunks = (p.K + TG_BK - 1) / TG_BK;
     p.rowvec_div = std::max(1, p.rowvec_div);
     if (p.rowvec_ld <= 0) p.rowvec_ld = p.N;
@@ -262,18 +265,19 @@ int star_linear_ex(const void* A, long long lda, const void* W, const void* bias
 
 int star_conv2d_3x3(const void* X, const void* W9, const void* bias, const void* rowvec, long long rowvec_div, long long ldrowvec,
                     const void* residual, long long ldres, void* out, long long ldo, int BT, int H, int W, int Cin,
-                    int Cout, void* stream) {
+                    int Cout, int row0, int H_out, void* stream) {
     STAR_CHECK_INIT();
     if (Cin % 8) return fail("star_conv2d_3x3: Cin must be a multiple of 8");
     if (rowvec && ldrowvec % 8) return fail("star_conv2d_3x3: ldrowvec must be a multiple of 8");
+    if (row0 < 0 || H_out < 1 || row0 + H_out > H) return fail("star_conv2d_3x3: output rows [%d, %d) outside [0, %d)", row0, row0 + H_out, H);
     TapGemmParams p{};
-    p.on[0] = W; p.on[1] = H; p.on[2] = BT; p.on[3] = 1;
-    conv_box(H, W, BT, p.box);
+    p.on[0] = W; p.on[1] = H_out; p.on[2] = BT; p.on[3] = 1;
+    conv_box(H_out, W, BT, p.box);
     p.ntaps = 9;
     for (int r = 0; r < 3; ++r)
         for (int s = 0; s < 3; ++s) {
             p.tap[r * 3 + s][0] = s - 1;
-            p.tap[r * 3 + s][1] = r - 1;
+            p.tap[r * 3 + s][1] = row0 + r - 1;
         }
     p.K = Cin; p.N = Cout;
     p.bias = (const __half*)bias; p.rowvec = (const __half*)rowvec; p.rowvec_div = (int)rowvec_div; p.rowvec_ld = ldrowvec;
@@ -324,21 +328,26 @@ int star_conv2d_3x3_s2p(const void* X, const void* W9, const void* bias, void* o
     return launch_tapgemm(p, planes_ws, Cin, W2, H2, 4, BT, W9, st);
 }
 
+// X holds pixels [p0, p0 + band) of every frame compactly ([B, T, band, Cin]); residual / out rows are those pixels of the
+// full [B, T, HW] row space (the tap-GEMM's row extents), so a pixel band of a clip-sized output is written in place.
 int star_conv_t3(const void* X, const void* W3, const void* bias, const void* residual, long long ldres, void* out,
-                 long long ldo, int B, int T, long long HW, int Cin, int Cout, void* stream) {
+                      long long ldo, int B, int T, long long HW, long long p0, long long band, int Cin, int Cout, void* stream) {
     STAR_CHECK_INIT();
     if (Cin % 8) return fail("star_conv_t3: Cin must be a multiple of 8");
     if (HW > 0x7fffffffll) return fail("star_conv_t3: HW too large");
+    if (p0 < 0 || band < 1 || p0 + band > HW) return fail("star_conv_t3: band [%lld, %lld) outside [0, %lld)", p0, p0 + band, HW);
     TapGemmParams p{};
-    p.on[0] = (int)HW; p.on[1] = T; p.on[2] = B; p.on[3] = 1;
-    p.box[0] = (int)std::min<long long>(TG_BM, HW); p.box[1] = 1; p.box[2] = 1; p.box[3] = 1;
-    if (HW < TG_BM) p.box[1] = (int)std::min<long long>(T, TG_BM / HW);     // small latents: several frames per tile
+    p.on[0] = (int)band; p.on[1] = T; p.on[2] = B; p.on[3] = 1;
+    p.row_ext[0] = (int)HW;
+    p.box[0] = (int)std::min<long long>(TG_BM, band); p.box[1] = 1; p.box[2] = 1; p.box[3] = 1;
+    if (band < TG_BM) p.box[1] = (int)std::min<long long>(T, TG_BM / band);     // small latents: several frames per tile
     p.ntaps = 3;
     for (int k = 0; k < 3; ++k) p.tap[k][1] = k - 1;
     p.K = Cin; p.N = Cout;
-    p.bias = (const __half*)bias; p.residual = (const __half*)residual; p.res_ld = ldres;
-    p.out = (__half*)out; p.out_ld = ldo;
-    return launch_tapgemm(p, X, Cin, HW, T, B, 1, W3, (cudaStream_t)stream);
+    p.bias = (const __half*)bias;
+    p.residual = residual ? (const __half*)residual + p0 * ldres : nullptr; p.res_ld = ldres;
+    p.out = (__half*)out + p0 * ldo; p.out_ld = ldo;
+    return launch_tapgemm(p, X, Cin, band, T, B, 1, W3, (cudaStream_t)stream);
 }
 
 // Causal Conv3d 3x3x3 of the CogVideoX 3-D VAE (cogvideox-based/sat/vae_modules/cp_enc_dec.py:360-430): X holds T + 2 frames --
@@ -480,32 +489,59 @@ long long star_groupnorm_workspace_bytes(int nsamples, int C) {
     return (long long)nsamples * 32 * 2 * 8 + (long long)nsamples * C * 2 * 4;
 }
 
-int star_groupnorm(const void* X, const void* gamma, const void* beta, void* out, int nsamples,
-                   long long rows_per_sample, int C, float eps, int silu, void* workspace, void* stream) {
+static Gn2Range gn2_range(int nsamples, long long rows_per_sample, unsigned& grid) {
+    Gn2Range rg;
+    rg.slabs_per_sample = (rows_per_sample + GN2_SLAB - 1) / GN2_SLAB;
+    rg.total_slabs = rg.slabs_per_sample * nsamples;
+    grid = (unsigned)std::min<long long>(rg.total_slabs, (long long)num_sms() * 8);
+    return rg;
+}
+
+// phases & STAR_GN_STATS: statistics + finalize into the workspace; phases & STAR_GN_APPLY: rows [p0, p0 + band) of every
+// frame_rows-row frame normalised with the workspace's (a, b) and written compactly to out (the whole sample: in place is fine)
+int star_groupnorm(const void* X, const void* gamma, const void* beta, void* out, int nsamples, long long rows_per_sample, int C,
+                   float eps, int silu, long long frame_rows, long long p0, long long band, int phases, void* workspace,
+                   void* stream) {
     if (C % 256 && C % 32) return fail("star_groupnorm: C must be a multiple of 32");
     if (C % 8) return fail("star_groupnorm: C must be a multiple of 8");
     if (C / 8 > GN_THREADS) return fail("star_groupnorm: C too large");
+    if (phases < 1 || phases > (STAR_GN_STATS | STAR_GN_APPLY)) return fail("star_groupnorm: phases must be 1, 2 or 3");
+    const bool whole = p0 == 0 && band == rows_per_sample && frame_rows == rows_per_sample;
+    if (frame_rows < 1 || rows_per_sample % frame_rows || p0 < 0 || band < 1 || p0 + band > frame_rows)
+        return fail("star_groupnorm: band [%lld, %lld) of %lld-row frames does not tile %lld-row samples", p0, p0 + band, frame_rows,
+                    rows_per_sample);
     cudaStream_t st = (cudaStream_t)stream;
     double* stats = (double*)workspace;
     float* ab = (float*)((char*)workspace + (size_t)nsamples * 32 * 2 * 8);
-    STAR_CUDA(cudaMemsetAsync(stats, 0, (size_t)nsamples * 32 * 2 * 8, st));
-    const long long total_rows = rows_per_sample * nsamples;
     if (C / 8 <= GN2_THREADS) {
         // persistent CTAs over contiguous slab ranges: statistics / (a, b) stay in registers across slabs
-        Gn2Range rg;
-        rg.slabs_per_sample = (rows_per_sample + GN2_SLAB - 1) / GN2_SLAB;
-        rg.total_slabs = rg.slabs_per_sample * nsamples;
-        const int lanes2 = GN2_THREADS / (C / 8);
-        const size_t smem2 = (size_t)lanes2 * C * 2 * sizeof(float);
-        const unsigned grid2 = (unsigned)std::min<long long>(rg.total_slabs, (long long)num_sms() * 8);
-        gn_stats2_kernel<<<grid2, GN2_THREADS, smem2, st>>>((const __half*)X, stats, rows_per_sample, C, rg);
-        STAR_LAUNCH_CHECK("gn_stats2");
-        gn_finalize_kernel<<<nsamples, 256, 0, st>>>(stats, (const __half*)gamma, (const __half*)beta, ab, rows_per_sample, C, eps);
-        STAR_LAUNCH_CHECK("gn_finalize");
-        gn_apply2_kernel<<<grid2, GN2_THREADS, 0, st>>>((const __half*)X, ab, (__half*)out, rows_per_sample, C, silu, rg);
-        STAR_LAUNCH_CHECK("gn_apply2");
+        unsigned grid2;
+        const Gn2Range rg = gn2_range(nsamples, rows_per_sample, grid2);
+        if (phases & STAR_GN_STATS) {
+            STAR_CUDA(cudaMemsetAsync(stats, 0, (size_t)nsamples * 32 * 2 * 8, st));
+            const int lanes2 = GN2_THREADS / (C / 8);
+            const size_t smem2 = (size_t)lanes2 * C * 2 * sizeof(float);
+            gn_stats2_kernel<<<grid2, GN2_THREADS, smem2, st>>>((const __half*)X, stats, rows_per_sample, C, rg);
+            STAR_LAUNCH_CHECK("gn_stats2");
+            gn_finalize_kernel<<<nsamples, 256, 0, st>>>(stats, (const __half*)gamma, (const __half*)beta, ab, rows_per_sample, C, eps);
+            STAR_LAUNCH_CHECK("gn_finalize");
+        }
+        if (!(phases & STAR_GN_APPLY)) return 0;
+        if (band == frame_rows) {
+            gn_apply2_kernel<<<grid2, GN2_THREADS, 0, st>>>((const __half*)X, ab, (__half*)out, rows_per_sample, C, silu, rg);
+            STAR_LAUNCH_CHECK("gn_apply2");
+            return 0;
+        }
+        const long long frames = (long long)nsamples * (rows_per_sample / frame_rows);
+        gn_apply_band_kernel<<<grid_for(frames * band * (C / 8), 256), 256, 0, st>>>((const __half*)X, ab, (__half*)out,
+                                                                                     rows_per_sample / frame_rows, frame_rows, p0,
+                                                                                     band, frames, C, silu);
+        STAR_LAUNCH_CHECK("gn_apply_band");
         return 0;
     }
+    if (phases != (STAR_GN_STATS | STAR_GN_APPLY) || !whole) return fail("star_groupnorm: C > 2048 runs both phases over whole samples");
+    STAR_CUDA(cudaMemsetAsync(stats, 0, (size_t)nsamples * 32 * 2 * 8, st));
+    const long long total_rows = rows_per_sample * nsamples;
     const int lanes = std::max(1, GN_THREADS / (C / 8));
     const size_t smem = (size_t)lanes * C * 2 * sizeof(float);
     dim3 grid((unsigned)((rows_per_sample + GN_SLAB - 1) / GN_SLAB), nsamples);

@@ -39,6 +39,9 @@ enum TapGemmFlags : int {
 
 struct TapGemmParams {
     int on[4];            // output extents n1..n4 (n1 fastest); rows_out = prod
+    int row_ext[4];       // extents of the output's row space (>= on; launch_tapgemm defaults them to on): a sub-box of a
+                          // larger row space, e.g. a pixel band of every frame, is written in place (out and residual;
+                          // launch_tapgemm refuses rowvec with extended extents)
     int box[4];           // tile box b1..b4, prod <= 128
     int tiles[4];         // ceil(on / box)
     int box_rows;         // prod(box)
@@ -166,7 +169,7 @@ STAR_DEVINL void tg_epilogue(const float (&acc)[BN / 2], const TapGemmParams& p,
             const int g = org[i] + l;
             ok = ok && (g < p.on[i]);
             orow += (long long)g * mul;
-            mul *= p.on[i];
+            mul *= p.row_ext[i];
         }
         valid[h] = ok;
         out_row[h] = p.out + orow * p.out_ld;

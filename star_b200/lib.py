@@ -23,10 +23,10 @@ SIGNATURES = {
     "star_linear_ex": (_i, [_p, _ll, _p, _p, _p, _ll, _p, _p, _ll, _p, _ll, _ll, _i, _i, _i, _p]),
     "star_row_gate": (_i, [_p, _p, _ll, _i, _i, _p, _f, _f, _p]),
     "star_qk_ln_rope": (_i, [_p, _ll, _ll, _i, _i, _p, _p, _p, _p, _p, _p, _i, _i, _f, _p]),
-    "star_conv2d_3x3": (_i, [_p, _p, _p, _p, _ll, _ll, _p, _ll, _p, _ll, _i, _i, _i, _i, _i, _p]),
+    "star_conv2d_3x3": (_i, [_p, _p, _p, _p, _ll, _ll, _p, _ll, _p, _ll, _i, _i, _i, _i, _i, _i, _i, _p]),
     "star_conv2d_s2_workspace_bytes": (_ll, [_i, _i, _i, _i]),
     "star_conv2d_3x3_s2": (_i, [_p, _p, _p, _p, _ll, _p, _i, _i, _i, _i, _i, _p]),
-    "star_conv_t3": (_i, [_p, _p, _p, _p, _ll, _p, _ll, _i, _i, _ll, _i, _i, _p]),
+    "star_conv_t3": (_i, [_p, _p, _p, _p, _ll, _p, _ll, _i, _i, _ll, _ll, _ll, _i, _i, _p]),
     "star_conv3d_causal": (_i, [_p, _p, _p, _p, _ll, _p, _ll, _i, _i, _i, _i, _i, _p]),
     "star_conv2d_c4_workspace_bytes": (_ll, [_i, _i, _i, _i]),
     "star_conv2d_3x3_c4": (_i, [_p, _p, _p, _p, _p, _p, _i, _i, _i, _i, _p]),
@@ -34,7 +34,7 @@ SIGNATURES = {
     "star_attention_causal": (_i, [_p, _ll, _p, _ll, _p, _ll, _p, _ll, _i, _i, _i, _f, _p]),
     "star_temporal_attention": (_i, [_p, _ll, _p, _ll, _i, _i, _ll, _i, _i, _f, _p]),
     "star_groupnorm_workspace_bytes": (_ll, [_i, _i]),
-    "star_groupnorm": (_i, [_p, _p, _p, _p, _i, _ll, _i, _f, _i, _p, _p]),
+    "star_groupnorm": (_i, [_p, _p, _p, _p, _i, _ll, _i, _f, _i, _ll, _ll, _ll, _i, _p, _p]),
     "star_groupnorm_mod": (_i, [_p, _p, _p, _p, _p, _ll, _p, _i, _i, _i, _i, _i, _i, _i, _f, _i, _p, _p]),
     "star_layernorm": (_i, [_p, _p, _p, _p, _ll, _i, _f, _i, _p, _f, _f, _p]),
     "star_liem_spatial_gate": (_i, [_p, _p, _p, _p, _i, _i, _i, _i, _p]),

@@ -16,6 +16,8 @@ HALF = torch.float16
 FLAG_GEGLU = 1
 FLAG_SILU_OUT = 2
 FLAG_GELU_ERF = 4
+GN_STATS = 1        # star_groupnorm phases
+GN_APPLY = 2
 
 
 # ---- optional per-op tracing (CUDA events on the launching stream) ---------------------------------
@@ -125,19 +127,21 @@ def linear(a, w, bias=None, residual=None, rowvec=None, rowvec_div=1, flags=0, o
 
 
 @_traced
-def conv2d_3x3(x, w9, bias=None, rowvec=None, rowvec_div=1, residual=None, out=None):
-    """x [BT, H, W, Cin] contiguous; w9 [Cout, 3, 3, Cin]; returns [BT*H*W, Cout]."""
+def conv2d_3x3(x, w9, bias=None, rowvec=None, rowvec_div=1, residual=None, out=None, rows=None):
+    """x [BT, H, W, Cin] contiguous; w9 [Cout, 3, 3, Cin]; returns [BT*H*W, Cout].  With rows=(row0, n) only output rows
+    row0..row0+n of each frame are computed ([BT*n*W, Cout]), their halo read from x."""
     L, dt = _bind(x)
     BT, H, W, Cin = x.shape
+    row0, Ho = (0, H) if rows is None else rows
     Cout = w9.shape[0]
     assert x.is_contiguous() and w9.is_contiguous() and w9.shape[1:] == (3, 3, Cin)
     if out is None:
-        out = torch.empty((BT * H * W, Cout), dtype=dt, device=x.device)
+        out = torch.empty((BT * Ho * W, Cout), dtype=dt, device=x.device)
     ldo = _rowmajor(out, "out")
     ldres = _rowmajor(residual, "residual") if residual is not None else 0
     ldrv = _rowmajor(rowvec, "rowvec") if rowvec is not None else 0           # a column slice of a wider matrix is fine
     _L.check(L, L.star_conv2d_3x3(_p(x), _p(w9), _p(bias), _p(rowvec), int(rowvec_div), ldrv, _p(residual), ldres,
-                                  _p(out), ldo, BT, H, W, Cin, Cout, _st()), "star_conv2d_3x3")
+                                  _p(out), ldo, BT, H, W, Cin, Cout, int(row0), int(Ho), _st()), "star_conv2d_3x3")
     return out
 
 
@@ -173,17 +177,21 @@ def conv2d_3x3_s2p(x, w9, bias=None, pad=(0, 1, 0, 1)):
 
 
 @_traced
-def conv_t3(x, w3, bias=None, residual=None, B=1, T=1, HW=1, out=None):
-    """Temporal conv (3,1,1): x [B*T*HW, Cin]; w3 [Cout, 3, Cin]."""
+def conv_t3(x, w3, bias=None, residual=None, B=1, T=1, HW=1, out=None, band=None):
+    """Temporal conv (3,1,1): x [B*T*HW, Cin]; w3 [Cout, 3, Cin].  With band=(p0, p1), x holds pixels p0..p1 of every frame
+    ([B*T*(p1-p0), Cin]) and only those rows of out / residual ([B*T*HW, .], out required) are read / written."""
     L, dt = _bind(x)
     rows, Cin = x.shape
-    assert rows == B * T * HW and x.is_contiguous() and w3.is_contiguous()
+    p0, p1 = (0, HW) if band is None else band
+    assert rows == B * T * (p1 - p0) and x.is_contiguous() and w3.is_contiguous()
     Cout = w3.shape[0]
     if out is None:
+        assert band is None, "conv_t3: a band is written into a given out"
         out = torch.empty((rows, Cout), dtype=dt, device=x.device)
+    assert out.shape[0] == B * T * HW and (residual is None or residual.shape[0] == B * T * HW)
     ldres = _rowmajor(residual, "residual") if residual is not None else 0
     _L.check(L, L.star_conv_t3(_p(x), _p(w3), _p(bias), _p(residual), ldres, _p(out), _rowmajor(out, "out"),
-                               B, T, HW, Cin, Cout, _st()), "star_conv_t3")
+                               B, T, HW, p0, p1 - p0, Cin, Cout, _st()), "star_conv_t3")
     return out
 
 
@@ -273,18 +281,37 @@ def temporal_attention(qkv, B, T, HW, heads, Ci, scale=0.125):
 
 
 @_traced
-def groupnorm(x, gamma, beta, nsamples, eps, silu, out=None):
-    """x [rows, C]; nsamples equal blocks of rows share statistics.  out may alias x (in place)."""
-    L, _ = _bind(x)
+def groupnorm(x, gamma, beta, nsamples, eps, silu, out=None, bands=None):
+    """x [rows, C]; nsamples equal blocks of rows share statistics.  out may alias x (in place).
+
+    With bands=(frame_rows, band) the statistics are taken once and an iterator is returned that yields ((p0, p1), y) for
+    consecutive pixel bands of every frame_rows-row frame, y = the normalised rows p0..p1 of every frame, compactly."""
+    L, dt = _bind(x)
     rows, C = x.shape
     assert x.is_contiguous() and rows % nsamples == 0
     ws = torch.empty(L.star_groupnorm_workspace_bytes(nsamples, C), dtype=torch.uint8, device=x.device)
+    per = rows // nsamples
+    if bands is not None:
+        _L.check(L, L.star_groupnorm(_p(x), _p(gamma), _p(beta), None, nsamples, per, C, float(eps), 0, per, 0, per, GN_STATS,
+                                     _p(ws), _st()), "star_groupnorm")
+        return _groupnorm_bands(L, dt, x, ws, nsamples, silu, *bands)
     if out is None:
         out = torch.empty_like(x)
     assert out.is_contiguous() and out.shape == x.shape
-    _L.check(L, L.star_groupnorm(_p(x), _p(gamma), _p(beta), _p(out), nsamples, rows // nsamples, C, float(eps),
-                                 int(bool(silu)), _p(ws), _st()), "star_groupnorm")
+    _L.check(L, L.star_groupnorm(_p(x), _p(gamma), _p(beta), _p(out), nsamples, per, C, float(eps), int(bool(silu)), per, 0, per,
+                                 GN_STATS | GN_APPLY, _p(ws), _st()), "star_groupnorm")
     return out
+
+
+def _groupnorm_bands(L, dt, x, ws, nsamples, silu, frame_rows, band):
+    rows, C = x.shape
+    for p0 in range(0, frame_rows, band):
+        p1 = min(frame_rows, p0 + band)
+        out = torch.empty((rows // frame_rows * (p1 - p0), C), dtype=dt, device=x.device)
+        _L.check(L, L.star_groupnorm(_p(x), None, None, _p(out), nsamples, rows // nsamples, C, 0.0, int(bool(silu)), frame_rows,
+                                     p0, p1 - p0, GN_APPLY, _p(ws), _st()), "star_groupnorm")
+        yield (p0, p1), out
+        del out
 
 
 @_traced

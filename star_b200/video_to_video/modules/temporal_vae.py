@@ -26,6 +26,7 @@ import json
 import math
 import os
 from types import SimpleNamespace
+from typing import NamedTuple
 
 import torch
 import torch.nn as nn
@@ -34,7 +35,95 @@ from ... import ops
 
 HALF = torch.float16
 
-__all__ = ["AutoencoderKLTemporalDecoder", "DiagonalGaussianDistribution"]
+__all__ = ["AutoencoderKLTemporalDecoder", "DecodePlan", "DiagonalGaussianDistribution", "decode_plan", "decode_peak_bytes"]
+
+
+# ---- decode plan ---------------------------------------------------------------------------------------------------------
+# A 3-frame window at 1080p -> 4x holds 26 GB per 128-channel full-resolution tensor, so decode() runs its full-resolution
+# stages a few frames at a time, each up block's upsample + conv a band of rows at a time, and its temporal convs a pixel
+# band at a time.  The window-sized tensors that the temporal GroupNorm statistics need (each st-resnet's input and output)
+# are not split; the plan bounds what one pass allocates on top of them.  It depends on the window's shape only, never on free
+# device memory, so a clip decodes the same way on any card.
+PASS_BYTES = 26 << 30           # one spatial pass's transient tensors: one 1080p -> 4x frame (24.2 GiB) fits, a 720p -> 4x window does not
+BAND_BYTES = 1 << 30            # one band of the normalised window / of an upsampled frame (split plans only)
+
+
+class DecodePlan(NamedTuple):
+    """frames: frames per pass of the spatial stages; band: pixels per band of the temporal stages; rows: output rows per band
+    of the upsample + conv (>= a stage's H*W / H: one band)."""
+    frames: int
+    band: int
+    rows: int
+
+
+def _stages(H, W, ch, layers):
+    """The decoder's st-resnets in order: (cin, cout, H, W of the input, upsample first?); the mid block's come first."""
+    top = ch[-1]
+    out = [(top, top, H, W, False) for _ in range(layers)]
+    prev, up = top, False
+    for c in reversed(ch):
+        for _ in range(layers + 1):
+            out.append((prev, c, H, W, up))
+            if up:
+                H, W, up = 2 * H, 2 * W, False
+            prev = c
+        up = True
+    return out
+
+
+def _pass_bytes(n, rows, cin, cout, H, W, up):
+    """transient bytes of one pass of _spatial over n frames (fp16): (upsample + conv, resnet)"""
+    hw2 = H * W * (4 if up else 1)
+    u = n * hw2 * cin * 2 if up else 0
+    if up:                                                    # the upsampled band: a whole pass, or rows + 4 rows of one frame
+        ub = u if rows >= 2 * H else min(2 * H, rows + 4) * 2 * W * cin * 2
+    t = n * hw2 * cin * 2 if cin == cout else 0               # GroupNorm output when x is the residual
+    return (u + ub if up else 0), u + t + n * hw2 * cout * 2
+
+
+def decode_plan(bf, num_frames, H, W, ch=(128, 256, 512, 512), layers=2):
+    """The plan decode() runs a window of bf latent frames of H x W under: all frames in one pass and one band when a pass
+    over the whole window stays within PASS_BYTES (every window up to 1080p outputs), else bands of BAND_BYTES and the most
+    frames per pass that stay within it."""
+    if bf < 1 or num_frames < 1 or bf % num_frames:
+        raise ValueError(f"decode_plan: bf={bf} is not a positive multiple of num_frames={num_frames}")
+    stages = _stages(H, W, ch, layers)
+    scale = 2 ** (len(ch) - 1)
+    full = DecodePlan(bf, H * W * scale * scale, H * scale)
+    if max(max(_pass_bytes(bf, full.rows, *s)) for s in stages) <= PASS_BYTES:
+        return full
+    band = min(full.band, max(128, BAND_BYTES // (2 * bf * max(ch)) // 128 * 128))
+    rows = min(full.rows, max(2, BAND_BYTES // (2 * W * scale * max(ch)) // 2 * 2))
+    frames = bf
+    while frames > 1 and max(max(_pass_bytes(frames, rows, *s)) for s in stages) > PASS_BYTES:
+        frames -= 1
+    return DecodePlan(frames, band, rows)
+
+
+def decode_peak_bytes(plan, bf, H, W, ch=(128, 256, 512, 512), layers=2):
+    """Predicted peak of the activations decode() allocates under `plan` (fp16 tensors and workspaces; weights and z excluded)."""
+    top, hw = ch[-1], H * W
+    rgb = bf * hw * 4 ** (len(ch) - 1) * 8 * 2                                        # held from the start
+    return rgb + _peak_without_rgb(plan, bf, H, W, ch, layers)
+
+
+def _peak_without_rgb(plan, bf, H, W, ch, layers):
+    top, hw = ch[-1], H * W
+    win = bf * hw * top * 2
+    peak = bf * hw * 4 * 2 + (bf * hw * 64 + top * 64) * 2 + win                      # conv_in: tokens, im2col, output
+    ld = (hw + 7) // 8 * 8
+    rb = max(128, min(hw, (1 << 28) // ld // 128 * 128))
+    peak = max(peak, 7 * win + (min(rb, hw) + top) * ld * 2)                          # mid-block attention
+    for cin, cout, h, w, up in _stages(H, W, ch, layers):
+        hw2 = h * w * (4 if up else 1)
+        x = bf * h * w * cin * 2
+        xs = 0 if not up and cin == cout else bf * hw2 * cout * 2
+        p_up, p_res = _pass_bytes(min(plan.frames, bf), plan.rows, cin, cout, h, w, up)
+        peak = max(peak, x + (xs if plan.frames < bf else 0) + p_up, x + xs + p_res)      # xs is allocated after pass 0's upsample
+        s = bf * hw2 * cout * 2
+        peak = max(peak, 2 * s + bf * min(plan.band, hw2) * cout * 2)                  # temporal: xs, t, one band of GN(xs)
+    hw = hw * 4 ** (len(ch) - 1)
+    return max(peak, bf * hw * (ch[0] + 3) * 2)                                       # tail: h, sample
 
 
 class DiagonalGaussianDistribution:
@@ -249,22 +338,76 @@ class AutoencoderKLTemporalDecoder(nn.Module):
 
     # ---- blocks (x: [n*H*W, C] fp16 tokens) ------------------------------------------------------------------
     @staticmethod
-    def _res2d(r, x, n, H, W, eps=1e-6):
-        cin = x.shape[1]
-        t = ops.groupnorm(x, r["n1"][0], r["n1"][1], n, eps, True)
+    def _res2d(r, x, n, H, W, out=None, eps=1e-6):
+        """x [n*H*W, cin] is consumed: with a shortcut conv the shortcut goes straight to out and x is then normalised in
+        place; without one x is the residual and out defaults to x itself (the last conv reads and writes the same element)."""
+        cin, cout = x.shape[1], r["c1"][0].shape[0]
+        if out is None:
+            out = x if "sc" not in r else torch.empty((x.shape[0], cout), dtype=HALF, device=x.device)
+        if "sc" in r:
+            res = ops.linear(x, r["sc"][0], r["sc"][1], out=out)
+            t = ops.groupnorm(x, r["n1"][0], r["n1"][1], n, eps, True, out=x)
+        else:
+            res = x
+            t = ops.groupnorm(x, r["n1"][0], r["n1"][1], n, eps, True)
         t = ops.conv2d_3x3(t.view(n, H, W, cin), r["c1"][0], r["c1"][1])
-        cout = t.shape[1]
         t = ops.groupnorm(t, r["n2"][0], r["n2"][1], n, eps, True, out=t)
-        sc = ops.linear(x, r["sc"][0], r["sc"][1]) if "sc" in r else x
-        return ops.conv2d_3x3(t.view(n, H, W, cout), r["c2"][0], r["c2"][1], residual=sc)
+        return ops.conv2d_3x3(t.view(n, H, W, cout), r["c2"][0], r["c2"][1], residual=res, out=out)
 
     @classmethod
-    def _st_res(cls, r, x, B, T, H, W):
-        xs = cls._res2d(r["s"], x, B * T, H, W)
-        t = ops.groupnorm(xs, r["tn1"][0], r["tn1"][1], B, 1e-5, True)
-        t = ops.conv_t3(t, r["tc1"][0], r["tc1"][1], B=B, T=T, HW=H * W)
+    def _spatial(cls, r, x, bf, H, W, frames, rows, up=None):
+        """Spatial half of a SpatioTemporalResBlock over the window x [bf*H*W, cin], `frames` frames per pass, preceded by the
+        previous up block's nearest-x2 upsample and conv (`rows` output rows per band) when `up` is given.  x is consumed.
+        Returns (xs, H', W')."""
+        cin, cout = x.shape[1], r["c1"][0].shape[0]
+        H2, W2 = (2 * H, 2 * W) if up is not None else (H, W)
+        hw, hw2 = H * W, H2 * W2
+        xs = x if up is None and "sc" not in r else None
+        for f0 in range(0, bf, frames):
+            n = min(frames, bf - f0)
+            xf = x[f0 * hw:(f0 + n) * hw]
+            if up is not None:
+                xf = cls._upconv(up, xf, n, H, W, rows)
+            if xs is None:              # after the first upsample: one pass over the window never holds xs and the upsample at once
+                xs = torch.empty((bf * hw2, cout), dtype=HALF, device=x.device)
+            cls._res2d(r, xf, n, H2, W2, out=xs[f0 * hw2:(f0 + n) * hw2])
+        return xs, H2, W2
+
+    @staticmethod
+    def _upconv(up, x, n, H, W, rows):
+        """conv3x3(nearest_x2(x)) of n frames x [n*H*W, C] -> [n*2H*2W, C].  With rows < 2H each frame is done in bands of
+        `rows` output rows (rows even): the band's input rows, plus one halo row on each side, are upsampled from x and the
+        conv computes only the band's rows, so at most rows + 4 upsampled rows of one frame exist at once."""
+        C, H2, W2 = x.shape[1], 2 * H, 2 * W
+        u = torch.empty((n * H2 * W2, C), dtype=HALF, device=x.device)
+        g = n if rows >= H2 else 1                  # frames per band
+        for j in range(0, n, g):
+            for r0 in range(0, H2, rows):
+                r1 = min(H2, r0 + rows)
+                a, b = max(0, r0 // 2 - 1), min(H, r1 // 2 + 1)         # low-res rows holding upsampled rows r0 - 1 .. r1
+                xu = ops.upsample2x(x[(j * H + a) * W:((j + g - 1) * H + b) * W], g, b - a, W)
+                kw = {} if r1 - r0 == H2 else {"rows": (r0 - 2 * a, r1 - r0)}      # a whole frame is the plain conv
+                ops.conv2d_3x3(xu.view(g, 2 * (b - a), W2, C), up[0], up[1], out=u[(j * H2 + r0) * W2:((j + g - 1) * H2 + r1) * W2],
+                               **kw)
+                del xu
+        return u
+
+    @staticmethod
+    def _temporal(r, xs, B, T, HW, band):
+        """Temporal half + AlphaBlender, in place on xs [B*T*HW, C].  The first GroupNorm's clip statistics are taken once;
+        its apply and the first (3,1,1) conv then run `band` pixels of every frame at a time, so only a band of the
+        normalised clip exists at once.  The second GroupNorm is in place and the second conv writes over its residual."""
+        t = torch.empty_like(xs)
+        if band >= HW:                  # one band: the same statistics and apply launches as the banded path
+            g = ops.groupnorm(xs, r["tn1"][0], r["tn1"][1], B, 1e-5, True)
+            ops.conv_t3(g, r["tc1"][0], r["tc1"][1], B=B, T=T, HW=HW, out=t)
+            del g
+        else:
+            for p01, g in ops.groupnorm(xs, r["tn1"][0], r["tn1"][1], B, 1e-5, True, bands=(HW, band)):
+                ops.conv_t3(g, r["tc1"][0], r["tc1"][1], B=B, T=T, HW=HW, band=p01, out=t)
+                del g
         t = ops.groupnorm(t, r["tn2"][0], r["tn2"][1], B, 1e-5, True, out=t)
-        return ops.conv_t3(t, r["tc2"][0], r["tc2"][1], residual=xs, B=B, T=T, HW=H * W)
+        return ops.conv_t3(t, r["tc2"][0], r["tc2"][1], residual=xs, B=B, T=T, HW=HW, out=xs)
 
     @staticmethod
     def _attention(a, x, n, HW):
@@ -321,32 +464,62 @@ class AutoencoderKLTemporalDecoder(nn.Module):
         return SimpleNamespace(latent_dist=dist) if return_dict else (dist,)
 
     @torch.no_grad()
-    def decode(self, z, num_frames, return_dict=True):
-        """z (b*num_frames, 4, h, w) -> sample (b*num_frames, 3, 8h, 8w) fp16."""
+    def decode(self, z, num_frames, return_dict=True, plan=None):
+        """z (b*num_frames, 4, h, w) -> sample (b*num_frames, 3, 8h, 8w) fp16.  Runs under decode_plan() of the window's
+        shape unless a DecodePlan is given; every plan computes the same function."""
         pk = self._packed()["dec"]
         bf, c, H, W = z.shape
         T = int(num_frames)
         if bf % T:
             raise ValueError("temporal VAE decode: batch is not a multiple of num_frames")
         B = bf // T
+        ch, L = self.config.block_out_channels, self.config.layers_per_block
+        plan = plan or decode_plan(bf, T, H, W, ch, L)
+        if plan.frames < 1 or plan.band < 1 or plan.rows < 2 or plan.rows % 2:
+            raise ValueError(f"temporal VAE decode: bad plan {plan}")
+
+        def stages():                   # (resnet, upsampler of the previous up block or None); "attn" = mid-block attention
+            yield pk["mid"][0], None
+            for r in pk["mid"][1:]:
+                yield "attn", None
+                yield r, None
+            up = None
+            for blk in pk["up"]:
+                for r in blk["res"]:
+                    yield r, up
+                    up = None
+                up = blk.get("up")
+
+        # A split plan's window-sized tensors come and go in caching-allocator segments of tens of GiB.  A small tensor carved
+        # from a freed one (this window's RGB or output, or the caller's post-processing of it) would pin it, and the next
+        # window could not place its own, so under a split plan the free cached segments are released before the small
+        # tensors are allocated and before returning.
+        scale = 2 ** (len(ch) - 1)
+        split = plan.frames < bf or plan.band < H * W * scale * scale or plan.rows < H * scale
+        if split:
+            torch.cuda.empty_cache()
+        rgb = torch.empty((bf * H * W * scale * scale, 8), dtype=HALF, device=z.device)
         h = ops.nchw5_to_tokens(z.float().unsqueeze(2))
         h = ops.conv2d_3x3_c4(h.view(bf, H, W, 4), pk["in"][0], pk["in"][1])
-        h = self._st_res(pk["mid"][0], h, B, T, H, W)
-        for r in pk["mid"][1:]:
-            h = self._attention(pk["attn"], h, bf, H * W)
-            h = self._st_res(r, h, B, T, H, W)
-        for blk in pk["up"]:
-            for r in blk["res"]:
-                h = self._st_res(r, h, B, T, H, W)
-            if "up" in blk:
-                C = h.shape[1]
-                h = ops.upsample2x(h, bf, H, W)
-                H, W = 2 * H, 2 * W
-                h = ops.conv2d_3x3(h.view(bf, H, W, C), blk["up"][0], blk["up"][1])
-        h = ops.groupnorm(h, pk["nout"][0], pk["nout"][1], bf, 1e-6, True, out=h)
-        rgb = torch.empty((bf * H * W, 8), dtype=HALF, device=h.device)
-        ops.conv2d_3x3(h.view(bf, H, W, h.shape[1]), pk["out"][0], pk["out"][1], out=rgb[:, :3])
+        for r, up in stages():
+            if isinstance(r, str):
+                h = self._attention(pk["attn"], h, bf, H * W)
+                continue
+            h, H, W = self._spatial(r["s"], h, bf, H, W, plan.frames, plan.rows, up)
+            h = self._temporal(r, h, B, T, H * W, plan.band)
+        HW = H * W
+        for f0 in range(0, bf, plan.frames):
+            n = min(plan.frames, bf - f0)
+            x = h[f0 * HW:(f0 + n) * HW]
+            x = ops.groupnorm(x, pk["nout"][0], pk["nout"][1], n, 1e-6, True, out=x)
+            ops.conv2d_3x3(x.view(n, H, W, h.shape[1]), pk["out"][0], pk["out"][1], out=rgb[f0 * HW:(f0 + n) * HW, :3])
+        del h
+        if split:
+            torch.cuda.empty_cache()
         sample = ops.vae_head(rgb, pk["head"][0], pk["head"][1], B, T, H, W)
+        del rgb
+        if split:
+            torch.cuda.empty_cache()
         return SimpleNamespace(sample=sample) if return_dict else (sample,)
 
     def forward(self, sample, sample_posterior=False, generator=None, num_frames=1):

@@ -12,8 +12,9 @@ torch.cuda.max_memory_allocated, untiled and with tiles of 90x160 latent pixels 
 and the pixel legs of a 720p -> 4x clip (2880x5120): time and peak memory of one frame's bilinear upsample + VAE encode and
 of one 3-frame VAE decode window (untiled VAE, synthetic weights), each with the share of its op time spent in the VAE's
 mid-block attention (a second, traced run), then enhance_frames(tile_size=(90, 160)) end to end on an 8-frame 720p clip with
-one solver step (skipped when a pixel leg fails; the failure is printed).
-python tools/tiled_bench.py [--frames 32] [--skip-e2e | --skip-latent]"""
+one solver step (skipped when a pixel leg fails or, from decode_peak_bytes, would not fit in 90 % of the free memory).  --lr 1080x1920 runs the pixel legs and
+enhance_frames of a 1080p -> 4x clip instead (4320x7680 on a 4368x7744 canvas; the decode window runs under a split plan).
+python tools/tiled_bench.py [--frames 32] [--skip-e2e | --skip-latent] [--lr 1080x1920]"""
 import argparse
 import os
 import sys
@@ -176,6 +177,14 @@ def pixel_legs(pipe, dev, lr=(720, 1280), scale=4):
         print(f"pixel {th}x{tw}: one frame upsample + encode failed: {e}", flush=True)
         return False
     zl = torch.randn(1, 4, 3, (th + pad[2] + pad[3]) // 8, (tw + pad[0] + pad[1]) // 8, device=dev)
+    from star_b200.video_to_video.modules.temporal_vae import decode_peak_bytes, decode_plan
+    torch.cuda.empty_cache()
+    need = decode_peak_bytes(decode_plan(3, 3, zl.shape[3], zl.shape[4]), 3, zl.shape[3], zl.shape[4])
+    free, _ = torch.cuda.mem_get_info(dev)
+    if need > 0.9 * free:
+        print(f"pixel {th}x{tw}: one 3-frame decode window not run (predicted {need / GB:.1f} GiB, {free / GB:.1f} GiB free)",
+              flush=True)
+        return False
 
     def decode():
         with torch.autocast("cuda"):
@@ -217,6 +226,8 @@ def main():
     ap.add_argument("--frames", type=int, default=32)
     ap.add_argument("--skip-e2e", action="store_true", help="latent legs only")
     ap.add_argument("--skip-latent", action="store_true", help="pixel legs and enhance_frames only")
+    ap.add_argument("--lr", default="720x1280", help="HxW of the low-resolution clip of the pixel legs and enhance_frames "
+                    "(1080x1920: 4320x7680 outputs on a 4368x7744 canvas)")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("tiled_bench needs a CUDA device")
@@ -233,8 +244,9 @@ def main():
         latent_legs(pipe, net, args.frames, dev)
     if not args.skip_e2e:
         pipe.vae = synth_vae(dev)
-        if pixel_legs(pipe, dev):
-            end_to_end(pipe, dev)
+        lr = tuple(int(v) for v in args.lr.split("x"))
+        if pixel_legs(pipe, dev, lr):
+            end_to_end(pipe, dev, lr=lr)
 
 
 if __name__ == "__main__":
