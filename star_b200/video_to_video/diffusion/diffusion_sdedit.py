@@ -16,7 +16,8 @@ step ("exact" mode: bit-identical stitching to the single-GPU loop, because
 the reference re-stitches all chunks every step, :330-353).  ``chunk_parallel=
 "literal"`` is the north-star wording (no per-step collective; each rank
 integrates its own chunk for all steps and the slices are gathered once at the
-end) -- it only equals the reference for single-chunk inputs.
+end) -- it only equals the reference for single-chunk inputs.  With spatial tiles (``tile_inds``) the (chunk, tile)
+windows are sharded instead, and their raw outputs are all-gathered one round of W windows at a time.
 """
 import random
 
@@ -156,7 +157,13 @@ class GaussianDiffusion(object):
         """Every solver-step evaluation runs the model on the windows of _windows -- the whole clip, or each chunk of
         ``chunk_inds`` -- and stitches the frames each window keeps into the clip's x0.  ``tile_inds`` (the output of
         video_to_video_model.make_tiles) turns on spatially tiled sampling: the windows are the (chunk, tile) pairs and
-        their x0 are blended into the clip's x0 with the tiles' weights (see _eval_x0_tiled)."""
+        their x0 are blended into the clip's x0 with the tiles' weights (see _eval_x0_tiled).
+
+        Under a process group of W > 1 ranks with ``chunk_parallel`` "auto" or "exact", tiled sampling shards the (chunk,
+        tile) windows round-robin, also for a single chunk, and exchanges their outputs round by round (_eval_x0_tiled): x0
+        is byte-identical to the single-process loop on every rank.  Every rank then applies the same solver update from
+        the same start: the SDE noise stream is seeded from rank 0 below, and denoise_latents broadcasts rank 0's diffused
+        latent.  "literal" with tiles is refused: it has no per-step exchange to blend with."""
         assert isinstance(steps, (int, torch.LongTensor))
         assert t_max is None or (0 < t_max <= self.num_timesteps - 1)
         assert t_min is None or (0 <= t_min < self.num_timesteps - 1)
@@ -176,14 +183,15 @@ class GaussianDiffusion(object):
         # SURVEY App. B); a one-window list is the un-chunked case.
         if chunk_inds is not None and len(chunk_inds) < 2:
             chunk_inds = None
-        if tile_inds is not None and _dist_info()[0] > 1:
-            raise NotImplementedError("sample_sr: tiled sampling runs in a single process; spatial tiles are not sharded "
-                                      "across ranks")
+        group = chunk_parallel in ("auto", "exact", "literal") and _dist_info()[0] > 1
+        if tile_inds is not None and group and chunk_parallel == "literal":
+            raise NotImplementedError("sample_sr(tile_inds=...): chunk_parallel='literal' has no per-step exchange to blend the "
+                                      "tiles with; use 'auto' or 'exact'")
 
         # Ranks of one job must integrate the same SDE path -- also for single-chunk clips, where every rank evaluates the whole
         # clip and the pipeline then shards only the VAE legs: share rank 0's noise seed whenever a process group exists.
-        group = chunk_parallel in ("auto", "exact", "literal") and _dist_info()[0] > 1
-        world, rank = _dist_info() if group and chunk_inds is not None else (1, 0)
+        # Tiled sampling shards its (chunk, tile) windows also for a single chunk.
+        world, rank = _dist_info() if group and (chunk_inds is not None or tile_inds is not None) else (1, 0)
         mode = "exact" if chunk_parallel == "auto" else chunk_parallel
         if group and solver == 'dpmpp_2m_sde' and kwargs.get('noise_sampler') is None:
             # every rank applies the same solver update: share the SDE noise stream (rank 0's seed)
@@ -194,8 +202,8 @@ class GaussianDiffusion(object):
 
         windows = self._windows(noise, chunk_inds, tile_inds, model_kwargs, guide_scale, clamp, percentile)
         # CFG-branch split (SURVEY 8e): with at least two ranks per chunk the (chunk, branch) pairs are the units --
-        # BASELINE config 3 (3 chunks) then fills 6 of 8 GPUs instead of 3.
-        split_cfg = (mode == "exact" and world >= 2 * len(windows) and isinstance(model_kwargs, list)
+        # BASELINE config 3 (3 chunks) then fills 6 of 8 GPUs instead of 3.  With tiles the units are the windows.
+        split_cfg = (tile_inds is None and mode == "exact" and world >= 2 * len(windows) and isinstance(model_kwargs, list)
                      and guide_scale not in (None, 1.0))
         wire = {}
         intermediates = []
@@ -204,7 +212,7 @@ class GaussianDiffusion(object):
             t, alphas, sigmas = self._t_coefs(xt, sigma)
             if tile_inds is not None:
                 x0 = self._eval_x0_tiled(xt, t, alphas, sigmas, windows, model, model_kwargs, guide_scale, guide_rescale,
-                                         variant_info)
+                                         variant_info, world, rank)
             elif split_cfg:
                 x0 = self._eval_x0_cfg_split(xt, t, alphas, sigmas, windows, model, model_kwargs, guide_scale,
                                              guide_rescale, variant_info, world, rank, wire)
@@ -300,25 +308,64 @@ class GaussianDiffusion(object):
             xt, model_kwargs = self._crop(xt, win), self._window_kwargs(model_kwargs, win)
         return xt, self._model_out(xt, t, model, model_kwargs, guide_scale, variant_info, branch)
 
-    def _eval_x0_tiled(self, xt, t, alphas, sigmas, windows, model, model_kwargs, guide_scale, guide_rescale, variant_info):
+    def _eval_x0_tiled(self, xt, t, alphas, sigmas, windows, model, model_kwargs, guide_scale, guide_rescale, variant_info,
+                       world=1, rank=0):
         """x0 of the clip = sum over (chunk, tile) windows of the tile's blend weight times its x0, restricted to the frames
         the chunk keeps (stitch_slices).  One star_cfg_x0_blend launch pair per window forms the guided x0 (CFG, std-ratio
         rescale over the window, v -> x0) and adds it into the clip's x0 in place.  Needs fp16 CUDA model outputs (the
-        .half() UNet)."""
+        .half() UNet).
+
+        On ``world`` ranks the windows run in rounds of ``world``: in round k rank r runs the model on window k * world + r,
+        one all-gather carries the round's raw model outputs (_gather_round), and every rank blends the round's windows in
+        window order.  The blends are those of the single-process loop, in its order, so x0 is byte-identical to it on every
+        rank; an all-reduce of partial sums would reorder them."""
         from ... import ops
         xt = xt.float().contiguous()
         x0 = torch.zeros_like(xt)
         rescale = None if guide_scale == 1.0 else guide_rescale        # as _x0: no rescale without a second branch
-        for win in windows:
-            out = self._window_out(xt, t, win, model, model_kwargs, guide_scale, variant_info)[1]
-            y_out, u_out = out if isinstance(out, tuple) else (out, out)
-            if not (y_out.is_cuda and y_out.dtype == torch.float16 and u_out.dtype == torch.float16):
-                raise TypeError("sample_sr(tile_inds=...): tiled sampling blends on the GPU and needs fp16 CUDA model outputs "
-                                f"(the .half() UNet), got {y_out.dtype} on {y_out.device}")
-            s, _, lo, hi, r0, _, c0, _, wy, wx = win
-            ops.cfg_x0(y_out.contiguous(), u_out.contiguous(), xt, alphas, sigmas, guide_scale, rescale,
-                       blend=ops.TileBlend(x0, s, lo, hi, r0, c0, wy, wx))
+        for k in range(0, len(windows), world):
+            wins = windows[k:k + world]
+            out = None
+            if rank < len(wins):
+                out = self._window_out(xt, t, wins[rank], model, model_kwargs, guide_scale, variant_info)[1]
+                y_out, u_out = out if isinstance(out, tuple) else (out, out)
+                if not (y_out.is_cuda and y_out.dtype == torch.float16 and u_out.dtype == torch.float16):
+                    raise TypeError("sample_sr(tile_inds=...): tiled sampling blends on the GPU and needs fp16 CUDA model "
+                                    f"outputs (the .half() UNet), got {y_out.dtype} on {y_out.device}")
+            outs = [out] if world == 1 else self._gather_round(out, wins, guide_scale != 1.0, xt)
+            for win, out in zip(wins, outs):
+                y_out, u_out = out if isinstance(out, tuple) else (out, out)
+                s, _, lo, hi, r0, _, c0, _, wy, wx = win
+                ops.cfg_x0(y_out.contiguous(), u_out.contiguous(), xt, alphas, sigmas, guide_scale, rescale,
+                           blend=ops.TileBlend(x0, s, lo, hi, r0, c0, wy, wx))
         return x0
+
+    @staticmethod
+    def _round_shape(wins, like, pair):
+        """The wire buffer of one round of tiled windows: (branches, B, C, frames, rows, cols), the round's largest extent
+        on each axis (chunks can differ in length), 2 branches under CFG with two model calls, else 1."""
+        b, c = like.shape[:2]
+        return ((2 if pair else 1), b, c, max(e - s for s, e, *_ in wins), max(w[5] - w[4] for w in wins),
+                max(w[7] - w[6] for w in wins))
+
+    @staticmethod
+    def _gather_round(out, wins, pair, like):
+        """ONE all-gather of a round of tiled windows' raw fp16 model outputs.  ``out`` is this rank's output -- the
+        (conditional, unconditional) pair when ``pair``, else one tensor -- or None when it has no window in the round, in
+        which case it sends only padding.  Returns the outputs of the round's windows in window order, cropped to each
+        window.  Device memory: one round of padded outputs, independent of the frame size."""
+        world, _ = _dist_info()
+        send = torch.zeros(GaussianDiffusion._round_shape(wins, like, pair), dtype=torch.float16, device=like.device)
+        if out is not None:
+            for dst, o in zip(send, out if pair else (out,)):
+                dst[:, :, :o.shape[2], :o.shape[3], :o.shape[4]] = o
+        recv = [torch.empty_like(send) for _ in range(world)]
+        dist.all_gather(recv, send)
+        outs = []
+        for (s, e, _, _, r0, r1, c0, c1, _, _), buf in zip(wins, recv):
+            o = tuple(x[:, :, :e - s, :r1 - r0, :c1 - c0] for x in buf)
+            outs.append(o if pair else o[0])
+        return outs
 
     # -- chunk-parallel helpers -------------------------------------------------
     def _eval_x0_cfg_split(self, xt, t, alphas, sigmas, windows, model, model_kwargs, guide_scale, guide_rescale,

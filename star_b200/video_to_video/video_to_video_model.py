@@ -17,10 +17,12 @@ Mirrors ``VideoToVideo_sr`` of the reference's video_to_video/video_to_video_mod
 * with ``torch.distributed`` initialised (one process per GPU) the whole entry is sharded (SURVEY 8e):
   - each rank uploads, upsamples and VAE-encodes only its contiguous share of the frames; the latents (0.42 MB per
     frame) are all-gathered, so every rank conditions on the SAME posterior sample (the reference draws it once);
-  - frame chunks -- or (chunk, CFG branch) pairs when there are at least two ranks per chunk -- are sharded across
-    ranks with one all-gather per solver step (diffusion_sdedit.GaussianDiffusion.sample_sr, ``chunk_parallel``);
-  - each rank decodes its share of the 3-frame VAE windows and ONE all-gather of the decoded, cropped frames
-    assembles the clip (the north-star's end collective).
+  - frame chunks -- or (chunk, CFG branch) pairs when there are at least two ranks per chunk, or (chunk, spatial tile)
+    windows with ``tile_size`` -- are sharded across ranks with all-gathers every solver step
+    (diffusion_sdedit.GaussianDiffusion.sample_sr, ``chunk_parallel``);
+  - test() decodes each rank's share of the 3-frame VAE windows and ONE all-gather of the decoded, cropped frames
+    assembles the clip (the north-star's end collective); enhance_frames decodes and colour-corrects the windows in
+    rounds of one window per rank, with one all-gather of the finished frames per round.
 """
 from typing import Any, Dict
 
@@ -162,20 +164,37 @@ class VideoToVideo_sr():
                        max_chunk_len=32, uint8=True, tile_size=None, tile_overlap=16):
         """test() + the CLI's post-processing (inference_sr.py:77-80: tensor2vid, adain_color_fix against the LR clip) with the
         post-processing on the GPU: returns (F, H, W, 3) frames in [0, 255] on the CPU -- uint8 by default, i.e. a quarter of the
-        device->host traffic of test()'s fp32 tensor.  In a single process the frames come from enhance_frames_iter, so the
-        device holds no whole-clip tensor at output resolution."""
-        if _dist_info()[0] == 1:
-            (h, w) = input['target_res']
-            out = torch.empty((input['video_data'].shape[0], h, w, 3), dtype=torch.uint8 if uint8 else torch.float32)
+        device->host traffic of test()'s fp32 tensor.  In a single process the frames come from enhance_frames_iter.  Under a
+        process group of W > 1 ranks the 3-frame decode windows run in rounds of W: in round k rank r decodes, crops and
+        colour-corrects window k * W + r, and one all-gather of the finished frames per round fills every rank's host tensor.
+        Either way the device holds no whole-clip tensor at output resolution."""
+        world, rank = _dist_info()
+        (h, w) = input['target_res']
+        out = torch.empty((input['video_data'].shape[0], h, w, 3), dtype=torch.uint8 if uint8 else torch.float32)
+        if world == 1:
             for s, frames in self.enhance_frames_iter(input, total_noise_levels, steps, solver_mode, guide_scale, max_chunk_len,
                                                       uint8, tile_size, tile_overlap):
                 out[s:s + frames.shape[0]] = frames
             return out
-        vid = self._test_on_device(input, total_noise_levels, steps, solver_mode, guide_scale, max_chunk_len,
-                                   tile_size, tile_overlap).float()
-        if vid.is_cuda:
-            return ops.adain_color_fix(vid, input['video_data'].to(vid.device).float(), uint8=uint8).cpu()
-        raise NotImplementedError("enhance_frames runs the GPU post-processing kernels; use test() + the reference's CPU helpers otherwise")
+        if torch.device(self.device).type != 'cuda':
+            raise NotImplementedError("enhance_frames runs the GPU post-processing kernels; use test() + the reference's CPU "
+                                      "helpers otherwise")
+        gen_vid, (w1, _, h1, _) = self._sample_latents(input, total_noise_levels, steps, solver_mode, guide_scale,
+                                                       max_chunk_len, tile_size, tile_overlap)
+        z = rearrange(gen_vid, "b c f h w -> (b f) c h w")
+        n, chunk_size = z.shape[0], 3
+        starts = list(range(0, n, chunk_size))
+        for k in range(0, len(starts), world):
+            rnd = starts[k:k + world]
+            if rank < len(rnd):
+                s = rnd[rank]
+                local = self._enhance_window(z, input['video_data'], s, min(chunk_size, n - s), (h1, h + h1, w1, w + w1),
+                                             uint8)
+            else:
+                local = torch.empty((0, h, w, 3), dtype=out.dtype, device=self.device)
+            frames = _all_gather_owned(local, [min(chunk_size, n - s) for s in rnd], 0)
+            out[rnd[0]:rnd[0] + frames.shape[0]] = frames
+        return out
 
     def enhance_frames_iter(self, input: Dict[str, Any], total_noise_levels=1000, steps=50, solver_mode='fast', guide_scale=7.5,
                             max_chunk_len=32, uint8=True, tile_size=None, tile_overlap=16):
@@ -207,14 +226,9 @@ class VideoToVideo_sr():
         stream = torch.cuda.current_stream(self.device)
 
         def launch(s):
-            """enqueue window [s, s + k): LR upload, decode (the windows and autocast of _test_on_device), crop, colour fix,
-            copy into a fresh pinned host tensor; returns (s, host tensor, device result, its copy's event)"""
-            k = min(chunk_size, n - s)
-            lr = self._upload_lr(video_data[s:s + k]).float()
-            with torch.autocast('cuda'):
-                dec = self.temporal_vae_decode(z[s:s + k], k)
-            vid = dec[:, :, h1:h + h1, w1:w + w1].permute(1, 0, 2, 3).unsqueeze(0).float()
-            out = ops.adain_color_fix(vid, lr, uint8=uint8)
+            """enqueue window [s, s + k) (_enhance_window) and its copy into a fresh pinned host tensor; returns (s, host
+            tensor, device result, its copy's event)"""
+            out = self._enhance_window(z, video_data, s, min(chunk_size, n - s), (h1, h + h1, w1, w + w1), uint8)
             host = torch.empty(out.shape, dtype=out.dtype, pin_memory=True)
             host.copy_(out, non_blocking=True)
             done = torch.cuda.Event()
@@ -231,6 +245,17 @@ class VideoToVideo_sr():
                 yield s, host
         finally:
             stream.synchronize()              # a caller that stops early leaves no work in flight
+
+    def _enhance_window(self, z, video_data, s, k, crop, uint8):
+        """Frames [s, s + k) of the clip, finished on the device: LR upload, decode of the latent frames z[s:s + k] ((b f) c h
+        w; the windows and autocast of _test_on_device), crop (t0, t1, l0, l1), colour fix against the LR frames.  Returns
+        (k, H, W, 3) in [0, 255], uint8 or fp32."""
+        t0, t1, l0, l1 = crop
+        lr = self._upload_lr(video_data[s:s + k]).float()
+        with torch.autocast('cuda'):
+            dec = self.temporal_vae_decode(z[s:s + k], k)
+        vid = dec[:, :, t0:t1, l0:l1].permute(1, 0, 2, 3).unsqueeze(0).float()
+        return ops.adain_color_fix(vid, lr, uint8=uint8)
 
     def _upload_lr(self, frames):
         """LR frames -> self.device.  A host tensor goes through pinned memory so that the copy is queued behind the work

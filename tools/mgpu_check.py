@@ -4,7 +4,10 @@
      ("exact" mode: chunks over ranks; with >= 2 ranks per chunk: (chunk, CFG branch) pairs)
   2. rank-local 3-frame VAE decode windows + ONE all-gather == single-GPU decode, bit for bit
   3. frame-sharded host upload + all-gather == direct upload
-  4. VideoToVideo_sr.test() sharded == every rank's own un-sharded run of the same entry (same seed)"""
+  4. VideoToVideo_sr.test() sharded == every rank's own un-sharded run of the same entry (same seed)
+  5. tiled denoise with the (chunk, tile) windows sharded round by round == the single-rank tiled loop, bit for bit
+  6. round-wise enhance_frames == test() + ops.adain_color_fix on the same ranks, byte for byte
+Exits non-zero when a check fails on any rank."""
 import os
 import sys
 
@@ -22,6 +25,7 @@ def main():
     dist.init_process_group("nccl", device_id=dev)
     from tests.test_vae import SMALL, _setup
     from tests.util import SMALL_KW, make_inputs, synth_model
+    from star_b200 import ops
     from star_b200.video_to_video.utils.seed import setup_seed
     from star_b200.video_to_video import video_to_video_model as M
     import logging
@@ -96,6 +100,32 @@ def main():
     print(f"[rank {rank}] test() sharded: every rank returns the identical video: {identical}; vs un-sharded run (different posterior-"
           f"sample RNG streams): rel-L2 {err:.3e}", flush=True)
     ok &= identical and out_sharded.shape == out_single.shape and bool(torch.isfinite(out_sharded).all())
+
+    # ---- 5. tiled denoise: 4 chunks x 2 tiles = 8 windows ("serial" keeps the whole tile loop on every rank)
+    xt, hint_t, yt = make_inputs(17, 1, 20, 26, 48)
+    noise_t = torch.randn(xt.shape, generator=torch.Generator().manual_seed(19)).to(dev)
+
+    def run_tiled(mode):
+        g = torch.Generator(device=dev).manual_seed(seeds[1])
+        sampler = lambda a, b: torch.randn(xt.shape, generator=g, device=dev)         # noqa: E731
+        return pipe.denoise_latents(hint_t.to(dev), yt.to(dev), -yt.to(dev), steps=2, solver_mode="normal", guide_scale=7.5,
+                                    max_chunk_len=8, noise=noise_t, noise_sampler=sampler, chunk_parallel=mode,
+                                    tile_size=(26, 32), tile_overlap=8)
+    same = torch.equal(run_tiled("serial"), run_tiled("auto"))
+    print(f"[rank {rank}] tiled denoise (8 windows on {world} ranks, round by round) == single-rank tiled run: {same}",
+          flush=True)
+    ok &= same
+
+    # ---- 6. round-wise enhance_frames (7 frames: 3 decode windows)
+    video = torch.rand(7, 3, 48, 64, generator=torch.Generator().manual_seed(23)) * 2 - 1
+    inp = {"video_data": video, "y": "a prompt", "target_res": (96, 128)}
+    setup_seed(666)
+    rounds = pipe.enhance_frames(inp, **kw)
+    setup_seed(666)
+    whole = ops.adain_color_fix(pipe.test(inp, **kw).to(dev), video.to(dev), uint8=True).cpu()
+    same = torch.equal(rounds, whole)
+    print(f"[rank {rank}] enhance_frames round by round == test() + colour fix: {same}", flush=True)
+    ok &= same
     flag = torch.tensor([1 if ok else 0], device=dev)
     dist.all_reduce(flag, op=dist.ReduceOp.MIN)
     dist.destroy_process_group()

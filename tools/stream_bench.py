@@ -3,8 +3,8 @@
 per clip length, on the full ControlledV2VUNet and the full temporal VAE (synthetic weights), one solver step:
 
   streamed    VideoToVideo_sr.enhance_frames_iter, every window consumed (the frames are dropped)
-  whole clip  _test_on_device + ops.adain_color_fix over the whole clip + one copy to the host (enhance_frames' multi-rank
-              body, run in one process)
+  whole clip  _test_on_device + ops.adain_color_fix over the whole clip + one copy to the host (test() + the colour fix,
+              which multi-rank enhance_frames equals byte for byte)
 
   240p -> 960p (LR 240x426, canvas 976x1728), F = 32, 96, 288
   480p -> 4x   (LR 480x854, canvas 1936x3456), tiles of 90x160 latent pixels, F = 32, 96
