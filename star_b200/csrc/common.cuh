@@ -169,6 +169,20 @@ STAR_DEVINL void tma_load_5d(void* dst, const CUtensorMap* m, uint64_t* bar, int
         "r"(c3), "r"(c4)
         : "memory");
 }
+// Store of a shared-memory box to global memory (clipped at the tensor map's extents), tracked in the issuing thread's
+// bulk async-groups: commit closes a group; bulk_wait_group_read<N> returns once at most N groups still read shared memory
+// (their source may then be overwritten), bulk_wait_group<N> once at most N groups are still writing global memory.
+STAR_DEVINL void tma_store_5d(const CUtensorMap* m, const void* src, int c0, int c1, int c2, int c3, int c4) {
+    asm volatile(
+        "cp.async.bulk.tensor.5d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5, %6}], [%1];"
+        ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
+        : "memory");
+}
+STAR_DEVINL void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+template <int N>
+STAR_DEVINL void bulk_wait_group_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+template <int N>
+STAR_DEVINL void bulk_wait_group() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
 
 // ---------------------------------------------------------------- misc math
 STAR_DEVINL float ex2_approx(float x);

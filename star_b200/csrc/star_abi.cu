@@ -102,30 +102,63 @@ int tile_width(int N, bool geglu) {
     return p160 <= p128 ? 160 : 128;
 }
 
+// The tensor maps of one tap-GEMM launch: the A and W operands and, for the staged epilogue, the output and residual
+// slabs (64 columns, and the 32-column tail of the 160-wide tile).  All of them together with TapGemmParams must fit the
+// 4 KB of kernel parameters.
+struct TapGemmMaps {
+    CUtensorMap a, w, out{}, res{}, out_tail{}, res_tail{};
+};
+static_assert(sizeof(TapGemmMaps) + sizeof(TapGemmParams) <= 4096, "tap-GEMM kernel parameters exceed 4 KB");
+
 // The epilogue instance compiled for exactly this call's epilogue kind, else the generic one.
-template <int BN>
-void launch_tapgemm_epi(const CUtensorMap& ta, const CUtensorMap& tw, const TapGemmParams& p, int grid, cudaStream_t st) {
+template <int BN, bool STAGED>
+void launch_tapgemm_epi(const TapGemmMaps& m, const TapGemmParams& p, int grid, cudaStream_t st) {
     const int kind = tg_epi_kind(p.flags, p.bias, p.rowvec, p.colscale, p.residual);
-    auto kernel = tapgemm_kernel<BN, TG_EPI_GENERIC>;
+    auto kernel = tapgemm_kernel<BN, TG_EPI_GENERIC, STAGED>;
 #define TG_EPI_CASE(K)                                                     \
     if constexpr ((K) != TG_EPI_GENERIC && tg_instance(BN, (K)))          \
-        if (kind == (K)) kernel = tapgemm_kernel<BN, (K)>;
+        if (kind == (K)) kernel = tapgemm_kernel<BN, (K), STAGED>;
     TG_EPI_KINDS(TG_EPI_CASE)
 #undef TG_EPI_CASE
-    kernel<<<grid, TG_THREADS, TapGemmSmem<BN>::TOTAL, st>>>(ta, tw, p);
+    kernel<<<grid, TG_THREADS, TapGemmSmem<BN, STAGED>::TOTAL, st>>>(m.a, m.w, m.out, m.res, m.out_tail, m.res_tail, p);
 }
 
-// Raises the dynamic shared-memory limit of instance <BN, EPI>, if it is compiled.
+// Raises the dynamic shared-memory limit of instance <BN, EPI> (both epilogue paths), if it is compiled.
 template <int BN, int EPI>
 int tapgemm_smem_attr() {
-    if constexpr (tg_instance(BN, EPI))
-        STAR_CUDA(cudaFuncSetAttribute(tapgemm_kernel<BN, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, TapGemmSmem<BN>::TOTAL));
+    if constexpr (tg_instance(BN, EPI)) {
+        STAR_CUDA(cudaFuncSetAttribute(tapgemm_kernel<BN, EPI, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       TapGemmSmem<BN, true>::TOTAL));
+        STAR_CUDA(cudaFuncSetAttribute(tapgemm_kernel<BN, EPI, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       TapGemmSmem<BN, false>::TOTAL));
+    }
     return 0;
+}
+
+// Whether TMA can address the slabs of an [rows, N] view with row pitch ld: a 16-byte-aligned base, and a row pitch and
+// a row length of whole 16-byte units (on an H100 a TMA store was seen to clip the inner extent only to 16 bytes: with
+// N % 8 != 0 it wrote past column N).  The staged epilogue needs it of the output and of the
+// residual; other calls take the direct one.
+bool tma_addressable(const void* base, long long ld, int N) {
+    return reinterpret_cast<uintptr_t>(base) % 16 == 0 && ld % 8 == 0 && N % 8 == 0;
+}
+
+// Tensor map of the output (or residual) slabs of a tile: (column, n1..n4) over the output extents, rows laid out over the
+// row extents, box = `cols` columns x the tile box.  TMA clips the box at the output extents and at N.
+int make_slab_tmap(CUtensorMap* m, const void* base, long long ld, const TapGemmParams& p, unsigned cols) {
+    unsigned long long dim[5] = {(unsigned long long)p.N}, str[5] = {1, (unsigned long long)ld};
+    unsigned box[5] = {cols};
+    for (int i = 0; i < 4; ++i) {
+        dim[i + 1] = (unsigned long long)p.on[i];
+        box[i + 1] = (unsigned)p.box[i];
+        if (i > 0) str[i + 1] = str[i] * (unsigned long long)p.row_ext[i - 1];
+    }
+    return make_tmap(m, base, 5, dim, str, box, cols == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B);
 }
 
 // Launches a tap-GEMM whose caller has filled p's output extents, box, taps, K, N, flags and epilogue inputs.  A holds
 // p.K channels per row, rows lda elements apart, viewed as extents n1..n4 (n1 fastest); W is [N (2N with GEGLU), ntaps * K].
-// Every other field of p, and both tensor maps, follow from those here.
+// Every other field of p, and the tensor maps, follow from those here.
 int launch_tapgemm(TapGemmParams& p, const void* A, unsigned long long lda, unsigned long long n1, unsigned long long n2,
                    unsigned long long n3, unsigned long long n4, const void* W, cudaStream_t st) {
     long long m_tiles = 1;
@@ -150,21 +183,31 @@ int launch_tapgemm(TapGemmParams& p, const void* A, unsigned long long lda, unsi
     if (total > 0x7fffffffll) return fail("tapgemm: too many tiles");
     p.num_tiles = (int)total;
 
-    CUtensorMap ta, tw;
+    TapGemmMaps m;
     unsigned long long adim[5] = {(unsigned long long)p.K, n1, n2, n3, n4}, astr[5] = {1, lda};
     for (int i = 2; i < 5; ++i) astr[i] = astr[i - 1] * adim[i - 1];
     unsigned abox[5] = {TG_BK, (unsigned)p.box[0], (unsigned)p.box[1], (unsigned)p.box[2], (unsigned)p.box[3]};
-    if (make_tmap(&ta, A, 5, adim, astr, abox)) return 1;
+    if (make_tmap(&m.a, A, 5, adim, astr, abox)) return 1;
     const unsigned long long wrows = geglu ? 2ull * p.N : (unsigned long long)p.N;
     unsigned long long wdim[2] = {(unsigned long long)p.ntaps * p.K, wrows};
     unsigned long long wstr[2] = {1, (unsigned long long)p.ntaps * p.K};
     unsigned wbox[2] = {TG_BK, (unsigned)n_per_tile};
-    if (make_tmap(&tw, W, 2, wdim, wstr, wbox)) return 1;
+    if (make_tmap(&m.w, W, 2, wdim, wstr, wbox)) return 1;
 
+    // The staged epilogue stores through TMA and loads the residual with it; the direct one serves the calls TMA cannot address.
+    const bool staged = tma_addressable(p.out, p.out_ld, p.N) && (!p.residual || tma_addressable(p.residual, p.res_ld, p.N));
+    if (staged) {
+        if (make_slab_tmap(&m.out, p.out, p.out_ld, p, 64)) return 1;
+        if (p.residual && make_slab_tmap(&m.res, p.residual, p.res_ld, p, 64)) return 1;
+        if (bn == 160) {
+            if (make_slab_tmap(&m.out_tail, p.out, p.out_ld, p, 32)) return 1;
+            if (p.residual && make_slab_tmap(&m.res_tail, p.residual, p.res_ld, p, 32)) return 1;
+        }
+    }
     const int grid = (int)std::min<long long>(total, num_sms());
-    if (bn == 256) launch_tapgemm_epi<256>(ta, tw, p, grid, st);
-    else if (bn == 160) launch_tapgemm_epi<160>(ta, tw, p, grid, st);
-    else launch_tapgemm_epi<128>(ta, tw, p, grid, st);
+    if (bn == 256) staged ? launch_tapgemm_epi<256, true>(m, p, grid, st) : launch_tapgemm_epi<256, false>(m, p, grid, st);
+    else if (bn == 160) staged ? launch_tapgemm_epi<160, true>(m, p, grid, st) : launch_tapgemm_epi<160, false>(m, p, grid, st);
+    else staged ? launch_tapgemm_epi<128, true>(m, p, grid, st) : launch_tapgemm_epi<128, false>(m, p, grid, st);
     STAR_LAUNCH_CHECK("tapgemm");
     return 0;
 }

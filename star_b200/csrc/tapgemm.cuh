@@ -16,8 +16,10 @@
 // Persistent kernel, one CTA per SM looping over 128 x BN output tiles (n fastest, so concurrently running CTAs
 // share the A tile in L2).  Warpgroup 0: one TMA producer thread filling a ring of (A, W) stages; warpgroups 1 and 2:
 // consumers, each computing 64 tile rows x BN columns with wgmma (fp32 accumulators in registers) and applying the
-// fused epilogue straight from registers.  The producer runs ahead into the next tile while the consumers finish the
-// epilogue of the current one.
+// fused epilogue.  The producer runs ahead into the next tile while the consumers finish the epilogue of the current one.
+// The staged epilogue (calls whose output and residual TMA can address) writes each tile through two shared-memory slabs
+// stored with TMA, without waiting for the writes; a second producer thread TMA-loads the residual into the slabs, the
+// first two slabs of a tile under its main loop.  The direct epilogue (other calls) stores from registers.
 #pragma once
 #include "common.cuh"
 #include "wgmma.cuh"
@@ -64,15 +66,20 @@ struct TapGemmParams {
     long long out_ld;
 };
 
-template <int BN>
+// Shared memory: the stage ring, then (staged epilogue) two output slabs of 128 rows x 64 columns, then the barriers.
+template <int BN, bool STAGED>
 struct TapGemmSmem {
     static constexpr int A_BYTES = TG_BM * TG_BK * 2;          // 16 KB
     static constexpr int B_BYTES = BN * TG_BK * 2;
     static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
+    static constexpr int SLAB_BYTES = TG_BM * 64 * 2;          // 16 KB, 1024-B aligned (STAGE_BYTES is a multiple of 1024)
+    static constexpr int SLABS = STAGED ? 2 : 0;
     static constexpr int MAX_STAGES = 8;
-    static constexpr int STAGES_FIT = (232448 - 1024 - 256) / STAGE_BYTES;     // 227 KB minus alignment slack and barriers
+    static constexpr int STAGES_FIT = (232448 - 1024 - 256 - SLABS * SLAB_BYTES) / STAGE_BYTES;  // 227 KB minus slabs, slack, barriers
     static constexpr int STAGES = STAGES_FIT < MAX_STAGES ? STAGES_FIT : MAX_STAGES;
-    static constexpr int TOTAL = STAGES * STAGE_BYTES + 1024 + 256;
+    static constexpr int SLAB_OFF = STAGES * STAGE_BYTES;
+    static constexpr int BAR_OFF = SLAB_OFF + SLABS * SLAB_BYTES;
+    static constexpr int TOTAL = BAR_OFF + 1024 + 256;
 };
 
 template <int BN>
@@ -251,24 +258,160 @@ STAR_DEVINL void tg_epilogue(const float (&acc)[BN / 2], const TapGemmParams& p,
     }
 }
 
+// Staged epilogue.  A tile's output columns are walked in slabs of 64 (the 128-wide tile: 2, 160: 64 + 64 + 32, 256: 4;
+// GEGLU at 256: 2, at 128: 1), alternating between two shared-memory slab buffers laid out as the output tensor maps'
+// boxes: box_rows rows of 128 B (the 32-column tail: 64 B) in the tile's row order, 128-byte (tail: 64-byte) swizzled.
+// Buffer b has a full barrier (the residual slab's TMA bytes) and an empty barrier (arrived by the thread that stored the
+// buffer's previous slab, once the store has read it).  The slabs of all tiles of a CTA are numbered in order; slab i
+// uses buffer i & 1 for the (i >> 1)-th time.
+STAR_DEVINL int tg_slab_count(const TapGemmParams& p, int n_per_tile, int n_base) {
+    return (min(n_per_tile, p.N - n_base) + 63) >> 6;
+}
+// Byte offset of (row r, slab column cc) in a slab buffer: SWIZZLE_128B on 128-byte rows, SWIZZLE_64B on the 64-byte rows
+// of the 32-column tail.  A warp's 8 rows of a column pair land in 8 different 16-B chunks: no bank conflicts.
+STAR_DEVINL uint32_t tg_slab_off(int r, int cc, bool tail) {
+    return tail ? (uint32_t)(r * 64 + cc * 2) ^ ((uint32_t)((r >> 1) & 3) << 4)
+                : (uint32_t)(r * 128 + cc * 2) ^ ((uint32_t)(r & 7) << 4);
+}
+STAR_DEVINL void tg_consumer_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+
+// Epilogue of one consumer warpgroup through the slab buffers.  Per slab: wait for the residual slab (or, without a
+// residual, for the buffer to be free), read each element's residual from the slab, apply the same fp32 sequence as
+// tg_epilogue, write the fp16 result over it in place, then one thread stores the slab with TMA (clipped at N and at the
+// output extents, so ragged tiles and sub-box writes need no masking) and moves on without waiting for the write.
 template <int BN, int EPI>
+STAR_DEVINL void tg_epilogue_staged(const float (&acc)[BN / 2], const TapGemmParams& p, const CUtensorMap* tm_out,
+                                    const CUtensorMap* tm_out_tail, uint8_t* slabs, uint64_t* slab_full,
+                                    uint64_t* slab_empty, uint32_t& slab_i, const int (&org)[4], int n_tile, int cw,
+                                    int row_in_wg, int q4) {
+    const TapGemmEpiOpts<EPI> o(p);
+    const int n_per_tile = o.geglu ? BN / 2 : BN;
+    const int n_base = n_tile * n_per_tile;
+    const int ns = tg_slab_count(p, n_per_tile, n_base);
+    int row[2];
+    bool valid[2];
+    const __half* rv_row[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int r = cw * 64 + row_in_wg + 8 * h;
+        int rr = r;
+        long long orow = 0, mul = 1;
+        bool ok = r < p.box_rows;
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const int l = rr % p.box[i];
+            rr /= p.box[i];
+            const int g = org[i] + l;
+            ok = ok && (g < p.on[i]);
+            orow += (long long)g * mul;
+            mul *= p.row_ext[i];
+        }
+        row[h] = r;
+        valid[h] = ok;
+        rv_row[h] = o.rowvec ? p.rowvec + (orow / p.rowvec_div) * p.rowvec_ld : nullptr;
+    }
+    constexpr int JH = BN / 16;                      // GEGLU: value column groups [0, JH), gate column groups [JH, 2 JH)
+#pragma unroll
+    for (int s = 0; s < (BN + 63) / 64; ++s) {
+        if (s >= ns) break;
+        const bool tail = BN == 160 && s == 2;       // the 32-column tail slab of the 160-wide tile
+        const int b = slab_i & 1;
+        const uint32_t use_parity = (slab_i >> 1) & 1;
+        uint8_t* slab = slabs + b * TapGemmSmem<BN, true>::SLAB_BYTES;
+        if (o.res) mbar_wait(&slab_full[b], use_parity);
+        else mbar_wait(&slab_empty[b], use_parity ^ 1);
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) {
+            const int j = 8 * s + jj;
+            if (j >= BN / 8) break;
+            if (o.geglu && j >= JH) break;
+            const int jg = j < JH ? j + JH : j;
+            const int cc = 8 * jj + 2 * q4;                  // slab column of this thread's pair
+            const int c = 64 * s + cc;                       // tile column
+            const int n = n_base + c;
+            if (c >= n_per_tile || n >= p.N) continue;
+            const int n1 = n + 1 < p.N ? n + 1 : n;          // clamped index for the loads of a lone last column
+            float bv[2] = {0.f, 0.f}, bg[2] = {0.f, 0.f}, cs[2] = {1.f, 1.f};
+            if (o.bias) {
+                bv[0] = tg_ld(p.bias + n);
+                bv[1] = tg_ld(p.bias + n1);
+                if (o.geglu) { bg[0] = tg_ld(p.bias + p.N + n); bg[1] = tg_ld(p.bias + p.N + n1); }
+            }
+            if (o.colscale) { cs[0] = tg_ld(p.colscale + n); cs[1] = tg_ld(p.colscale + n1); }
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                if (!valid[h]) continue;
+                uint32_t* sp = reinterpret_cast<uint32_t*>(slab + tg_slab_off(row[h], cc, tail));
+                float f[2];
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    float x = acc[4 * j + 2 * h + e];
+                    if (o.geglu) {
+                        float g = acc[4 * jg + 2 * h + e];
+                        if (o.bias) { x += bv[e]; g += bg[e]; }
+                        x *= gelu_erf_f(g);
+                    } else if (o.bias) {
+                        x += bv[e];
+                    }
+                    if (o.tanh) x = gelu_tanh_f(x);
+                    if (o.erf) x = gelu_erf_f(x);
+                    if (o.colscale) x *= cs[e];
+                    if (o.rowvec) x += tg_ld(rv_row[h] + (e ? n1 : n));
+                    f[e] = x;
+                }
+                if (o.res) {           // not contracted with a product before it: tg_epilogue adds it in a block of its own
+                    const uint32_t r2 = *sp;
+                    const float2 rv = __half22float2(*reinterpret_cast<const __half2*>(&r2));
+                    f[0] = __fadd_rn(f[0], rv.x);
+                    f[1] = __fadd_rn(f[1], rv.y);
+                }
+                if (o.silu) { f[0] = silu_f(f[0]); f[1] = silu_f(f[1]); }
+                *sp = pack_half2(f[0], f[1]);
+            }
+        }
+        fence_proxy_async_smem();                    // the slab's generic writes, before the async proxy reads them
+        tg_consumer_sync();
+        if (threadIdx.x == TG_THREADS / 3) {         // first consumer thread: issues every store of the CTA
+            tma_store_5d(tail ? tm_out_tail : tm_out, slab, n_base + 64 * s, org[0], org[1], org[2], org[3]);
+            bulk_commit_group();
+            bulk_wait_group_read<0>();
+            mbar_arrive(&slab_empty[b]);
+        }
+        ++slab_i;
+    }
+}
+
+template <int BN, int EPI, bool STAGED>
 __global__ void __launch_bounds__(TG_THREADS, 1)
 tapgemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_w,
+               const __grid_constant__ CUtensorMap tmap_out, const __grid_constant__ CUtensorMap tmap_res,
+               const __grid_constant__ CUtensorMap tmap_out_tail, const __grid_constant__ CUtensorMap tmap_res_tail,
                const __grid_constant__ TapGemmParams p) {
-    using SM = TapGemmSmem<BN>;
+    using SM = TapGemmSmem<BN, STAGED>;
     uint8_t* smem = dyn_smem_1024();
-    StageRing<SM::STAGES> ring(reinterpret_cast<uint64_t*>(smem + SM::STAGES * SM::STAGE_BYTES));
+    StageRing<SM::STAGES> ring(reinterpret_cast<uint64_t*>(smem + SM::BAR_OFF));
+    uint8_t* slabs = smem + SM::SLAB_OFF;
+    uint64_t* slab_full = reinterpret_cast<uint64_t*>(smem + SM::BAR_OFF) + 2 * SM::STAGES;
+    uint64_t* slab_empty = slab_full + 2;
 
     const int wg = threadIdx.x >> 7;
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
-    const bool geglu = TapGemmEpiOpts<EPI>(p).geglu;
+    const TapGemmEpiOpts<EPI> opts(p);
+    const bool geglu = opts.geglu;
     const int total_iters = p.ntaps * p.k_chunks;
 
     if (threadIdx.x == 0) {
         tma_prefetch_desc(&tmap_a);
         tma_prefetch_desc(&tmap_w);
         ring.init(TG_CONSUMER_WARPS);
+        if constexpr (STAGED) {
+            tma_prefetch_desc(&tmap_out);
+            for (int b = 0; b < 2; ++b) {
+                mbar_init(&slab_full[b], 1);
+                mbar_init(&slab_empty[b], 1);
+            }
+        }
         fence_barrier_init();
     }
     __syncthreads();
@@ -312,6 +455,25 @@ tapgemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
                     }
                 }
             }
+        } else if (STAGED && opts.res && threadIdx.x == 32) {
+            // ------------------------------------------------ residual producer: each tile's residual slabs, in the
+            // consumers' slab order, as soon as their buffer is free (the first two of a tile arrive under its main loop)
+            const int n_per_tile = geglu ? BN / 2 : BN;
+            uint32_t slab_i = 0;
+            for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+                int org[4], n_tile;
+                tile_origin(tile, org, n_tile);
+                const int n_base = n_tile * n_per_tile;
+                const int ns = tg_slab_count(p, n_per_tile, n_base);
+                for (int s = 0; s < ns; ++s, ++slab_i) {
+                    const int b = slab_i & 1;
+                    const bool tail = BN == 160 && s == 2;
+                    mbar_wait(&slab_empty[b], ((slab_i >> 1) & 1) ^ 1);
+                    mbar_expect_tx(&slab_full[b], (uint32_t)p.box_rows * (tail ? 64u : 128u));
+                    tma_load_5d(slabs + b * SM::SLAB_BYTES, tail ? &tmap_res_tail : &tmap_res, &slab_full[b], n_base + 64 * s,
+                                org[0], org[1], org[2], org[3]);
+                }
+            }
         }
         return;
     }
@@ -324,6 +486,7 @@ tapgemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
     const uint64_t desc_a0 = wgmma_desc_sw128(smem_u32(smem) + cw * 64 * 128, 16, 1024);
     const uint64_t desc_b0 = wgmma_desc_sw128(smem_u32(smem) + SM::A_BYTES, 16, 1024);
     constexpr uint64_t STAGE_INC = (uint64_t)(SM::STAGE_BYTES >> 4);
+    uint32_t slab_i = 0;
     for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
         int org[4], n_tile;
         tile_origin(tile, org, n_tile);
@@ -348,8 +511,13 @@ tapgemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
         wgmma_wait<0>();
         if (prev_s >= 0) ring.release(prev_s);
 
-        tg_epilogue<BN, EPI>(acc, p, org, n_tile, cw, row_in_wg, q4);
+        if constexpr (STAGED)
+            tg_epilogue_staged<BN, EPI>(acc, p, &tmap_out, &tmap_out_tail, slabs, slab_full, slab_empty, slab_i, org, n_tile,
+                                        cw, row_in_wg, q4);
+        else
+            tg_epilogue<BN, EPI>(acc, p, org, n_tile, cw, row_in_wg, q4);
     }
+    if (STAGED && threadIdx.x == TG_THREADS / 3) bulk_wait_group<0>();      // the stores have written global memory
 }
 
 }  // namespace star

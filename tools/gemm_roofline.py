@@ -63,6 +63,48 @@ def epi_instance(flags, epi):
     return k if k in EPI_INSTANCES else EPI_GENERIC
 
 
+# epilogue path (star_abi.cu: launch_tapgemm, tma_addressable): the staged epilogue, which stores the output and loads the
+# residual through TMA, runs when TMA can address both: a 16-byte-aligned base, and a row pitch and N that are multiples
+# of 8 elements.  Other calls take the direct epilogue, which stores from registers.
+def tma_addressable(offset_bytes, ld, n):
+    """offset_bytes: of the view's first element from a 16-byte-aligned allocation (torch's CUDA allocator aligns to 512 B)"""
+    return offset_bytes % 16 == 0 and ld % 8 == 0 and n % 8 == 0
+
+
+def staged_epilogue(n, out_offset_bytes, out_ld, res_offset_bytes=None, res_ld=None):
+    """whether a call with N = n columns runs the staged epilogue (no residual: res_ld None)"""
+    return tma_addressable(out_offset_bytes, out_ld, n) and (res_ld is None or tma_addressable(res_offset_bytes, res_ld, n))
+
+
+def call_epilogue_views(name, fn, args, kwargs):
+    """(N, (offset bytes, ld) of the output, the same of the residual or None) of one ops.<name> call, as the library sees
+    them; None for a call the wrapper refuses (a view whose columns are not contiguous)"""
+    b = inspect.signature(fn).bind(*args, **kwargs)
+    b.apply_defaults()
+    a = b.arguments
+
+    def view(t, cols):
+        if t is None:                                    # allocated by the wrapper: [rows, cols], contiguous
+            return 0, cols
+        if t.dim() != 2 or t.stride(1) != 1:             # refused by the wrapper (ops._rowmajor): no launch
+            return None
+        return t.storage_offset() * t.element_size(), t.stride(0)
+    flags = int(a.get("flags", 0) or 0)
+    if name in ("linear", "linear_ex"):
+        n = a["w"].shape[0] // (2 if flags & 1 else 1)
+    else:
+        n = a[{"conv_t3": "w3", "conv3d_causal": "w27"}.get(name, "w9")].shape[0]
+    out = view(a.get("out"), n)
+    res = view(a["residual"], n) if a.get("residual") is not None else None
+    if out is None or (res is None and a.get("residual") is not None):
+        return None
+    if name == "conv_t3" and a.get("band") is not None:  # star_conv_t3 offsets out / residual to the band's first pixel
+        p0 = int(a["band"][0])
+        out = (out[0] + p0 * out[1] * 2, out[1])
+        res = None if res is None else (res[0] + p0 * res[1] * 2, res[1])
+    return n, out, res
+
+
 def best_box_2d(h, w):
     """conv_box: the (h, w) box of at most 128 pixels that covers h x w in the fewest tiles, the wider on a tie"""
     best, th, tw = -1, 1, 1
