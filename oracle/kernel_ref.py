@@ -358,14 +358,17 @@ def conv3d_causal(xp, w27, T, H, W, bias=None, residual=None, out=None):
 
 
 def spatial_norm_src_index(T, H, W, Tl, Hl, Wl, device):
-    """row (t, h, w) -> latent row, the nearest-neighbour rule of SpatialNorm3D.forward (cp_enc_dec.py:492-500)"""
-    t = torch.arange(T, device=device)
+    """row (t, h, w) -> latent row, the nearest-neighbour rule of SpatialNorm3D.forward (cp_enc_dec.py:492-500): each index
+    is F.interpolate(mode="nearest")'s min(floor(dst * s), n_in - 1) with the fp32 scale s = n_in / n_out"""
+    def nearest(n_out, n_in):
+        s = torch.tensor(n_in, dtype=torch.float32) / torch.tensor(n_out, dtype=torch.float32)
+        i = (torch.arange(n_out, device=device, dtype=torch.float32) * s.to(device)).floor().long()
+        return i.clamp(max=n_in - 1)
     if T > 1 and T % 2 == 1:
-        ts = torch.where(t == 0, torch.zeros_like(t), 1 + ((t - 1) * (Tl - 1)) // max(T - 1, 1))
+        ts = torch.cat([torch.zeros(1, dtype=torch.long, device=device), 1 + nearest(T - 1, Tl - 1)])
     else:
-        ts = (t * Tl) // T
-    hs = (torch.arange(H, device=device) * Hl) // H
-    ws = (torch.arange(W, device=device) * Wl) // W
+        ts = nearest(T, Tl)
+    hs, ws = nearest(H, Hl), nearest(W, Wl)
     return ((ts[:, None, None] * Hl + hs[None, :, None]) * Wl + ws[None, None, :]).reshape(-1)
 
 

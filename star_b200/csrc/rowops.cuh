@@ -395,12 +395,21 @@ __global__ void gn_apply_band_kernel(const __half* __restrict__ x, const float* 
 // GroupNorm apply of the CogVideoX 3-D VAE's SpatialNorm3D (cp_enc_dec.py:451-510): y = GN(x) * Y[src] + B[src] (+ SiLU), where
 // Y = conv_y(zq), B = conv_b(zq) are 1x1x1 convolutions of the latent and therefore commute with the nearest-neighbour
 // interpolation of zq to the feature size: they are evaluated ONCE at latent resolution (Tl, Hl, Wl) and gathered per row.
-// Row r = (t, h, w) of the (T, H, W) clip reads latent row (ts, h*Hl/H, w*Wl/W); ts follows the reference's split of the first
-// frame when T is odd (> 1): ts = 0 for t = 0, else 1 + (t-1)(Tl-1)/(T-1); otherwise ts = t*Tl/T.  One sample (B = 1).
+// Row r = (t, h, w) of the (T, H, W) clip reads latent row (ts, hs, ws), each index F.interpolate(mode="nearest")'s:
+// src = min(floor(dst * s), n_in - 1) with the fp32 scale s = n_in / n_out.  For a ratio whose fp32 reciprocal rounds low
+// (41, 47, 55, 61, ...) that is one less than dst * n_in / n_out at some multiples of the ratio, so exact integer division
+// would read the wrong latent row.  ts follows the reference's split of the first frame when T is odd (> 1): ts = 0 for t = 0,
+// else 1 + the nearest index of t - 1 from Tl - 1 to T - 1 frames.  One sample (B = 1).
 struct GnModGeom {
     int T, H, W, Tl, Hl, Wl, split_first;
     int hshift, wshift;       // log2(H / Hl), log2(W / Wl) when those ratios are powers of two (the VAE's: 1, 2, 4, 8), else -1
+    float tscale, hscale, wscale;   // fp32 source / destination size ratios, computed on the host (T: of the split's rest)
 };
+
+// F.interpolate(mode="nearest")'s source index of destination index dst
+STAR_DEVINL int nearest_src(int dst, float scale, int n_in) {
+    return min((int)floorf(__fmul_rn((float)dst, scale)), n_in - 1);
+}
 
 __global__ void __launch_bounds__(GN2_THREADS)
 gn_apply_mod_kernel(const __half* __restrict__ x, const float* __restrict__ ab, const __half* __restrict__ ymod,
@@ -424,8 +433,8 @@ gn_apply_mod_kernel(const __half* __restrict__ x, const float* __restrict__ ab, 
     }
     const int H = gm.H, W = gm.W, HW = H * W;
     auto t_src = [&](int t) {
-        if (gm.split_first) return t == 0 ? 0 : 1 + ((t - 1) * (gm.Tl - 1)) / (gm.T - 1);
-        return (t * gm.Tl) / gm.T;
+        if (gm.split_first) return t == 0 ? 0 : 1 + nearest_src(t - 1, gm.tscale, gm.Tl - 1);
+        return nearest_src(t, gm.tscale, gm.Tl);
     };
     // one division set per slab, then (t, h, w) advance incrementally: the row index arithmetic must not outweigh 48 bytes of traffic
     for (long long g = g0; g < g1; ++g) {
@@ -444,8 +453,8 @@ gn_apply_mod_kernel(const __half* __restrict__ x, const float* __restrict__ ab, 
             for (int k = 0; k < 4; ++k) {
                 rr[k] = r < r1 ? r : -1;
                 if (rr[k] >= 0) {
-                    const int hs = gm.hshift >= 0 ? (h >> gm.hshift) : (h * gm.Hl) / H;
-                    const int ws = gm.wshift >= 0 ? (w >> gm.wshift) : (w * gm.Wl) / W;
+                    const int hs = gm.hshift >= 0 ? (h >> gm.hshift) : nearest_src(h, gm.hscale, gm.Hl);
+                    const int ws = gm.wshift >= 0 ? (w >> gm.wshift) : nearest_src(w, gm.wscale, gm.Wl);
                     const long long src = ((long long)(ts * gm.Hl + hs) * gm.Wl + ws) * ldmod + oc * 8;
                     ux[k] = __ldg(reinterpret_cast<const uint4*>(x + (long long)r * C + oc * 8));
                     uy[k] = __ldg(reinterpret_cast<const uint4*>(ymod + src));

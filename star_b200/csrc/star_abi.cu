@@ -610,11 +610,12 @@ int star_groupnorm_mod(const void* X, const void* gamma, const void* beta, const
     const bool split = T > 1 && (T & 1);
     if (split ? ((T - 1) % std::max(1, Tl - 1) != 0 || Tl < 2) : (T % Tl != 0))
         return fail("star_groupnorm_mod: T=%d is not an integer multiple of the latent T=%d", T, Tl);
+    const long long rows = (long long)T * H * W;
+    if (rows > 0x7fffffffll) return fail("star_groupnorm_mod: more than 2^31 rows");
     cudaStream_t st = (cudaStream_t)stream;
     double* stats = (double*)workspace;
     float* ab = (float*)((char*)workspace + (size_t)32 * 2 * 8);
     STAR_CUDA(cudaMemsetAsync(stats, 0, (size_t)32 * 2 * 8, st));
-    const long long rows = (long long)T * H * W;
     Gn2Range rg;
     rg.slabs_per_sample = (rows + GN2_SLAB - 1) / GN2_SLAB;
     rg.total_slabs = rg.slabs_per_sample;
@@ -625,9 +626,11 @@ int star_groupnorm_mod(const void* X, const void* gamma, const void* beta, const
     STAR_LAUNCH_CHECK("gn_stats2");
     gn_finalize_kernel<<<1, 256, 0, st>>>(stats, (const __half*)gamma, (const __half*)beta, ab, rows, C, eps);
     STAR_LAUNCH_CHECK("gn_finalize");
-    if (rows > 0x7fffffffll) return fail("star_groupnorm_mod: more than 2^31 rows");
     auto log2_exact = [](int q) { int s = 0; while ((1 << s) < q) ++s; return (1 << s) == q ? s : -1; };
-    GnModGeom gm{T, H, W, Tl, Hl, Wl, split ? 1 : 0, log2_exact(H / Hl), log2_exact(W / Wl)};
+    // the scales F.interpolate computes (fp32 source / destination sizes), here on the host: device division is approximate
+    const float tscale = split ? (float)(Tl - 1) / (float)(T - 1) : (float)Tl / (float)T;
+    GnModGeom gm{T, H, W, Tl, Hl, Wl, split ? 1 : 0, log2_exact(H / Hl), log2_exact(W / Wl), tscale, (float)Hl / (float)H,
+                 (float)Wl / (float)W};
     gn_apply_mod_kernel<<<grid2, GN2_THREADS, 0, st>>>((const __half*)X, ab, (const __half*)Ymod, (const __half*)Bmod,
                                                        ldmod, (__half*)out, rows, C, silu, rg, gm);
     STAR_LAUNCH_CHECK("gn_apply_mod");

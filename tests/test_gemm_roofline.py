@@ -24,6 +24,26 @@ def test_roofline_restates_the_dispatch():
         assert (m["bn"], m["tiles"], m["iters"]) == (case.bn, pl.tiles, pl.iters), case.id
 
 
+def test_geometry_of_row_and_pixel_bands():
+    """conv2d_3x3(rows=(row0, n)) boxes its n output rows (star_abi.cu: on[1] = H_out, conv_box(H_out, W, BT)); conv_t3(band=
+    (p0, p1)) tiles p1 - p0 pixels, box[0] = min(128, band) and several frames per box under 128 (on[0] = band), and reads
+    only the band's rows of the clip; hand-computed"""
+    conv = dict(BT=2, H=13, W=24, Cin=64, Cout=64)
+    assert R.geometry("conv2d_3x3", conv)[:2] == ((24, 13, 2, 1), (24, 5, 1, 1))
+    assert R.geometry("conv2d_3x3", dict(conv, rows=(5, 2)))[:2] == ((24, 2, 2, 1), (24, 2, 2, 1))
+    assert R.geometry("conv2d_3x3", dict(conv, BT=3, W=40, rows=(0, 1)))[:2] == ((40, 1, 3, 1), (40, 1, 3, 1))
+    assert R.geometry("conv2d_3x3", dict(conv, BT=1, H=40, W=300, rows=(10, 4)))[:2] == ((300, 4, 1, 1), (64, 2, 1, 1))
+    assert R.geometry("conv2d_3x3", dict(conv, rows=(5, 2)))[5] == 2 * 13 * 24             # the whole frame is read
+    t3 = dict(B=2, T=5, HW=50, Cin=64, Cout=64)
+    assert R.geometry("conv_t3", t3)[:2] == ((50, 5, 2, 1), (50, 2, 1, 1))
+    assert R.geometry("conv_t3", dict(t3, band=(9, 37)))[::5] == ((28, 5, 2, 1), 2 * 5 * 50)   # the clip's rows
+    assert R.band_input_rows("conv_t3", dict(t3, band=(9, 37))) == 2 * 5 * 28                 # read compactly
+    assert R.band_input_rows("conv_t3", t3) == R.band_input_rows("conv2d_3x3", dict(conv, BT=1, H=10, W=50)) == 500
+    assert R.geometry("conv_t3", dict(t3, band=(9, 37)))[1] == (28, 4, 1, 1)
+    assert R.geometry("conv_t3", dict(t3, HW=500, T=3, band=(0, 300)))[:2] == ((300, 3, 2, 1), (128, 1, 1, 1))
+    assert R.geometry("conv_t3", dict(t3, HW=90, T=3, band=(89, 90)))[:2] == ((1, 3, 2, 1), (1, 3, 1, 1))
+
+
 def test_roofline_arithmetic():
     conv = R.Shape("conv2d_3x3", tuple(sorted(dict(BT=32, H=122, W=216, Cin=320, Cout=320).items())), 0, ("bias",))
     m = R.model(conv)

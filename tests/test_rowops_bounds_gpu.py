@@ -79,20 +79,26 @@ def _temporal_gate(x64, w0, w1, n_lane, dtype):
 B = "tests.test_kernel_bounds_gpu::"
 S = "tests.test_spatial_tiles_gpu::"
 R = "tests.test_rowops_bounds_gpu::"
+N = "tests.test_banded_bounds_gpu::"
 COVERAGE = {
     "star_linear": [(B + "test_tapgemm_bound", "fp16,bf16")],
     "star_linear_ex": [(B + "test_tapgemm_bound", "fp16,bf16")],
-    "star_conv2d_3x3": [(B + "test_tapgemm_bound", "fp16,bf16")],
+    "star_conv2d_3x3": [(B + "test_tapgemm_bound", "fp16,bf16"), (N + "test_conv2d_3x3_rows_bound", "fp16,bf16"),
+                        (N + "test_conv2d_3x3_rows_past_2_32_elements", "fp16")],
     "star_conv2d_3x3_s2": [(R + "test_conv2d_s2_bound", "fp16")],
     "star_conv2d_3x3_s2p": [(B + "test_tapgemm_bound", "fp16"), (R + "test_vae_convs_bf16_bound", "bf16")],
-    "star_conv_t3": [(B + "test_tapgemm_bound", "fp16")],
+    "star_conv_t3": [(B + "test_tapgemm_bound", "fp16"), (N + "test_conv_t3_band_bound", "fp16,bf16"),
+                     (N + "test_conv_t3_band_past_2_31_elements", "fp16")],
     "star_conv2d_3x3_c4": [(R + "test_conv2d_c4_bound", "fp16")],
     "star_attention": [(B + "test_attention_bound", "fp16,bf16")],
     "star_attention_causal": [(B + "test_attention_causal_bound", "fp16")],
     "star_temporal_attention": [(B + "test_temporal_attention_bound", "fp16")],
     "star_conv3d_causal": [(B + "test_tapgemm_bound", "fp16"), (R + "test_vae_convs_bf16_bound", "bf16")],
-    "star_groupnorm": [(B + "test_groupnorm_offset_bound", "fp16"), (R + "test_groupnorm_bf16_bound", "bf16")],
-    "star_groupnorm_mod": [(B + "test_groupnorm_mod_offset_bound", "fp16"), (R + "test_groupnorm_mod_bf16_bound", "bf16")],
+    "star_groupnorm": [(B + "test_groupnorm_offset_bound", "fp16"), (R + "test_groupnorm_bf16_bound", "bf16"),
+                       (N + "test_groupnorm_bands_bound", "fp16,bf16"), (N + "test_groupnorm_bands_refuses_C_above_2048", "fp16"),
+                       (N + "test_groupnorm_past_2_32_elements", "fp16")],
+    "star_groupnorm_mod": [(B + "test_groupnorm_mod_offset_bound", "fp16"), (R + "test_groupnorm_mod_bf16_bound", "bf16"),
+                           (N + "test_groupnorm_mod_geometry_bound", "fp16,bf16")],
     "star_layernorm": [(B + "test_layernorm_offset_bound", "fp16"), (R + "test_layernorm_gate_bound", "fp16"),
                        (R + "test_layernorm_bf16_bound", "bf16")],
     "star_liem_spatial_gate": [(R + "test_liem_spatial_gate_bound", "fp16,bf16")],
@@ -102,13 +108,15 @@ COVERAGE = {
     "star_add": [(R + "test_add_exact", "fp16")],
     "star_upsample2x_crop": [(R + "test_upsample2x_exact", "fp16,bf16")],
     "star_time_avgpool2": [(R + "test_time_avgpool2_bound", "fp16,bf16")],
-    "star_upsample2x": [(R + "test_upsample2x_exact", "fp16,bf16")],
+    "star_upsample2x": [(R + "test_upsample2x_exact", "fp16,bf16"), (N + "test_upsample2x_past_2_32_elements", "fp16")],
     "star_softmax_rows": [(R + "test_softmax_rows_bound", "fp16"), (R + "test_softmax_rows_refuses_102401_columns", "fp16")],
-    "star_vae_head": [(R + "test_vae_head_bound", "fp16")],
+    "star_vae_head": [(R + "test_vae_head_bound", "fp16"), (N + "test_vae_head_and_tokens_to_nchw5_past_2_32_elements", "fp16")],
     "star_nchw5_to_tokens": [(R + "test_layout_conversions_exact", "fp16,bf16")],
-    "star_tokens_to_nchw5": [(R + "test_layout_conversions_exact", "fp16,bf16")],
+    "star_tokens_to_nchw5": [(R + "test_layout_conversions_exact", "fp16,bf16"),
+                             (N + "test_vae_head_and_tokens_to_nchw5_past_2_32_elements", "fp16")],
     "star_bilinear_pad": [(R + "test_bilinear_pad_bound", "fp32")],
-    "star_adain_color_fix": [(R + "test_adain_color_fix_bound", "fp32,uint8"), (R + "test_adain_refuses_too_many_planes", "fp32")],
+    "star_adain_color_fix": [(R + "test_adain_color_fix_bound", "fp32,uint8"), (R + "test_adain_refuses_too_many_planes", "fp32"),
+                             (N + "test_adain_color_fix_past_2_31_elements", "uint8")],
     "star_cfg_x0": [(R + "test_cfg_x0_exact", "fp16")],
     "star_cfg_x0_blend": [(S + "test_blend_unit_weights_bit_exact", "fp16")],
     "star_sinusoidal": [(R + "test_sinusoidal_bound", "fp16,bf16")],

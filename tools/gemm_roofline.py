@@ -119,12 +119,16 @@ def best_box_2d(h, w):
 
 
 def geometry(op, d):
-    """(output extents on[4], box[4], taps, K, N, input rows) of one entry point, as it fills TapGemmParams"""
+    """(output extents on[4], box[4], taps, K, N, input rows) of one entry point, as it fills TapGemmParams.  conv2d_3x3 with
+    d["rows"] = (row0, n): output rows row0..row0+n of every frame, boxed over n rows (the whole frames are the input);
+    conv_t3 with d["band"] = (p0, p1): pixels p0..p1 of every frame.  Input rows are those of the whole clip, B T HW, also for
+    a band, whose call reads the band's B T (p1 - p0) of them, compactly (band_input_rows)."""
     if op in ("linear", "linear_ex"):
         return (d["rows"], 1, 1, 1), (128, 1, 1, 1), 1, d["K"], d["N"], d["rows"]
     if op == "conv2d_3x3":
-        th, tw = best_box_2d(d["H"], d["W"])
-        return ((d["W"], d["H"], d["BT"], 1), (tw, th, max(1, min(d["BT"], 128 // (tw * th))), 1), 9, d["Cin"], d["Cout"],
+        ho = d["rows"][1] if d.get("rows") is not None else d["H"]
+        th, tw = best_box_2d(ho, d["W"])
+        return ((d["W"], ho, d["BT"], 1), (tw, th, max(1, min(d["BT"], 128 // (tw * th))), 1), 9, d["Cin"], d["Cout"],
                 d["BT"] * d["H"] * d["W"])
     if op in ("conv2d_3x3_s2", "conv2d_3x3_s2p"):
         pt, pb, pl, pr = d.get("pad", (2, 2, 1, 1))
@@ -132,14 +136,22 @@ def geometry(op, d):
         th, tw = best_box_2d(ho, wo)
         return (wo, ho, 1, d["BT"]), (tw, th, 1, 1), 9, d["Cin"], d["Cout"], d["BT"] * d["H"] * d["W"]
     if op == "conv_t3":
-        hw, t = d["HW"], d["T"]
+        t = d["T"]
+        hw = d["band"][1] - d["band"][0] if d.get("band") is not None else d["HW"]
         return ((hw, t, d["B"], 1), (min(128, hw), min(t, 128 // hw) if hw < 128 else 1, 1, 1), 3, d["Cin"], d["Cout"],
-                d["B"] * t * hw)
+                d["B"] * t * d["HW"])
     if op == "conv3d_causal":
         th, tw = best_box_2d(d["H"], d["W"])
         return ((d["W"], d["H"], d["T"], 1), (tw, th, max(1, min(d["T"], 128 // (tw * th))), 1), 27, d["Cin"], d["Cout"],
                 (d["T"] + 2) * d["H"] * d["W"])
     raise ValueError(op)
+
+
+def band_input_rows(op, d):
+    """rows of the A operand one call reads: a conv_t3 band is passed compactly ([B T (p1 - p0), Cin]), other calls read
+    geometry()'s input rows"""
+    on, _, _, _, _, rows_in = geometry(op, d)
+    return math.prod(on) if op == "conv_t3" else rows_in
 
 
 def m_tiles(on, box):
@@ -168,10 +180,14 @@ def shape_of_call(name, fn, args, kwargs):
         d = {"BT": int(BT), "H": int(H), "W": int(W), "Cin": int(Cin), "Cout": int(a["w9"].shape[0])}
         if name == "conv2d_3x3_s2p":
             d["pad"] = tuple(int(v) for v in a["pad"])
+        if name == "conv2d_3x3" and has("rows"):
+            d["rows"] = tuple(int(v) for v in a["rows"])
         if has("rowvec"):
             d["rv_div"] = int(a["rowvec_div"])
     elif name == "conv_t3":
         d = {"B": int(a["B"]), "T": int(a["T"]), "HW": int(a["HW"]), "Cin": int(a["x"].shape[1]), "Cout": int(a["w3"].shape[0])}
+        if has("band"):
+            d["band"] = tuple(int(v) for v in a["band"])
     else:
         d = {"T": int(a["T"]), "H": int(a["H"]), "W": int(a["W"]), "Cin": int(a["xp"].shape[1]), "Cout": int(a["w27"].shape[0])}
     epi = tuple(k for k in ("bias", "rowvec", "colscale", "residual") if has(k))
@@ -201,7 +217,7 @@ def model(shape, sms=NUM_SMS):
     tiles = m_tiles(on, box) * _ceil(N, npt)
     iters = taps * _ceil(K, 64)
     flops = 2.0 * M * taps * K * wrows
-    hbm = 2.0 * (rows_in * K + wrows * taps * K + M * N)
+    hbm = 2.0 * (band_input_rows(shape.op, d) * K + wrows * taps * K + M * N)
     if "residual" in shape.epi:
         hbm += 2.0 * M * N
     if "rowvec" in shape.epi:
@@ -241,12 +257,13 @@ def make_call(O, shape):
     on, box, taps, K, N, rows_in = geometry(shape.op, d)
     wrows = 2 * N if shape.flags & 1 else N
     M = math.prod(on)
+    M_out = rows_in if shape.op == "conv_t3" else M                             # a band is written into the whole clip
     rnd = lambda *s, scale=1.0: (torch.randn(*s, device="cuda") * scale).half()  # noqa: E731
     bias = rnd(wrows, scale=0.1) if "bias" in shape.epi else None
-    res = rnd(M, N) if "residual" in shape.epi else None
+    res = rnd(M_out, N) if "residual" in shape.epi else None
     rv = rnd(_ceil(M, d.get("rv_div", 1)), N) if "rowvec" in shape.epi else None
     cs = rnd(N) if "colscale" in shape.epi else None
-    out = torch.empty(M, N, dtype=torch.float16, device="cuda")
+    out = torch.empty(M_out, N, dtype=torch.float16, device="cuda")
     sc = (taps * K) ** -0.5
     if shape.op == "linear":
         a, w = rnd(M, K), rnd(wrows, K, scale=sc)
@@ -256,7 +273,7 @@ def make_call(O, shape):
         return lambda: O.linear_ex(a, w, bias, cs, res, shape.flags, out=out)
     if shape.op == "conv2d_3x3":
         x, w = rnd(d["BT"], d["H"], d["W"], K), rnd(N, 3, 3, K, scale=sc)
-        return lambda: O.conv2d_3x3(x, w, bias, rv, d.get("rv_div", 1), res, out=out)
+        return lambda: O.conv2d_3x3(x, w, bias, rv, d.get("rv_div", 1), res, out=out, rows=d.get("rows"))
     if shape.op == "conv2d_3x3_s2":
         x, w = rnd(d["BT"], d["H"], d["W"], K), rnd(N, 3, 3, K, scale=sc)
         return lambda: O.conv2d_3x3_s2(x, w, bias)
@@ -265,7 +282,7 @@ def make_call(O, shape):
         return lambda: O.conv2d_3x3_s2p(x, w, bias, d["pad"])
     if shape.op == "conv_t3":
         x, w = rnd(M, K), rnd(N, 3, K, scale=sc)
-        return lambda: O.conv_t3(x, w, bias, res, d["B"], d["T"], d["HW"], out=out)
+        return lambda: O.conv_t3(x, w, bias, res, d["B"], d["T"], d["HW"], out=out, band=d.get("band"))
     x, w = rnd(rows_in, K), rnd(N, 3, 3, 3, K, scale=sc)
     return lambda: O.conv3d_causal(x, w, d["T"], d["H"], d["W"], bias, res, out=out)
 
