@@ -42,10 +42,15 @@ int star_linear(const void* A, long long lda, const void* W, const void* bias, c
 
 /* star_linear with a per-output-column scale applied before the residual add:
  * out = residual + colscale[n] * (acc + bias[n])  -- the adaLN gates of the CogVideoX DiT layer
- * (cogvideox-based/sat/dit_video_concat.py:543-544,:560-561).  flags may also carry STAR_FLAG_GELU_TANH. */
+ * (cogvideox-based/sat/dit_video_concat.py:543-544,:560-561).  flags may also carry STAR_FLAG_GELU_TANH.
+ * a_block_cols > 0: A is head-blocked, row r of A being K / a_block_cols blocks of a_block_cols columns side by side, block
+ * b of row r at A + b * a_block_pitch + r * lda (the attention output a token-sharded DiT rank gets back from its head
+ * all-to-all, star_b200/cogvideox/parallel.py); a_block_cols a multiple of 64 dividing K, at most 27 blocks, no GEGLU.  The
+ * result is the unblocked call's on the concatenated rows, bit for bit.  a_block_cols = 0: A is [rows, lda]. */
 int star_linear_ex(const void* A, long long lda, const void* W, const void* bias, const void* rowvec,
                    long long rowvec_div, const void* colscale, const void* residual, long long ldres, void* out,
-                   long long ldo, long long rows, int K, int N, int flags, void* stream);
+                   long long ldo, long long rows, int K, int N, int flags, int a_block_cols, long long a_block_pitch,
+                   void* stream);
 
 /* Conv2d 3x3 stride 1 pad 1 on X[BT,H,W,Cin]; W9 = weight permuted to [Cout][3][3][Cin]; rowvec = per-clip time
  * embedding added before the next GroupNorm; replaces cuDNN at unet_v2v.py:612,:639,:553-554,:1552.  Only output rows
@@ -127,9 +132,12 @@ int star_groupnorm_mod(const void* X, const void* gamma, const void* beta, const
 int star_layernorm(const void* X, const void* gamma, const void* beta, void* out, long long rows, int C, float eps,
                    int gate_mode, const void* gate, float w0, float w1, void* stream);
 /* Spatial LIEM gate: channel max/mean -> 7x7 conv (2->1) -> sigmoid (unet_v2v.py:380-394).  w98 = conv1.weight
- * flattened [2][7][7]; mm_ws = scratch rows*2 fp16; gate = rows fp16. */
+ * flattened [2][7][7]; mm_ws = the clip's channel max/mean map [BT*H*W][2] fp16.  Runs over tokens [r0, r0 + n) of the clip
+ * (r0 = 0, n = BT*H*W: the whole clip): X (NULL: skipped) holds those tokens' rows [n, C], and their max/mean go to
+ * mm_ws rows [r0, r0 + n); gate (NULL: skipped) receives their n gates, from mm_ws over the whole clip.  A token-sharded
+ * DiT rank reduces its own tokens, all-gathers the map and gates its own tokens. */
 int star_liem_spatial_gate(const void* X, const void* w98, void* mm_ws, void* gate, int BT, int H, int W, int C,
-                           void* stream);
+                           long long r0, long long n, void* stream);
 
 /* CogVideoX DiT layer helpers (cogvideox-based/sat/dit_video_concat.py).
  * star_row_gate: out = X * g(row); mode 1: g = gate[row] (spatial LIEM, :523-527, gate from star_liem_spatial_gate);

@@ -162,7 +162,11 @@ class DiffusionTransformer(nn.Module):
         return pk
 
     @torch.no_grad()
-    def forward(self, x, timesteps=None, context=None, y=None, **unused):
+    def forward(self, x, timesteps=None, context=None, y=None, shard=None, **unused):
+        """shard: this rank's parallel.SeqShard to run the layers token-sharded over its group (see parallel.py); the
+        returned output is the whole one on every rank of the group"""
+        if shard is not None:
+            return self._forward_shard(x, timesteps, context, shard)
         pk = self._pk if self._pk is not None else self._pack()
         c, dt = self.cfg, self.dtype
         b, t, cin, hh, ww = x.shape
@@ -198,3 +202,45 @@ class DiffusionTransformer(nn.Module):
             ops.linear(img, *pk["lin_f"], out=out[bi * n_img:(bi + 1) * n_img])
         co = c["out_channels"]                                                     # "b (t h w) (c p q) -> b t c (h p) (w q)"
         return out.view(b, t, gh, gw, co, p, p).permute(0, 1, 4, 2, 5, 3, 6).reshape(b, t, co, gh * p, gw * p)
+
+    def _forward_shard(self, x, timesteps, context, sp):
+        """``forward`` with the token rows sp.me of every sample on this rank; one all-gather of the image-token outputs at
+        the end hands every rank the whole output"""
+        pk = self._pk if self._pk is not None else self._pack()
+        c, dt, me = self.cfg, self.dtype, sp.me
+        b, t, cin, hh, ww = x.shape
+        p, d, tl = c["patch"], c["hidden"], self.text_length
+        gh, gw = hh // p, ww // p
+        assert (t, gh, gw) == (self.frames, self.gh, self.gw) and cin == 2 * c["in_channels"] and context.shape[1] == tl
+        n_img, n, nt, ni = t * gh * gw, me.rows, me.text_rows, me.image_rows
+        i0 = me.start + nt - tl                                                     # first image token of the shard
+        # ---- embeddings of the shard's text and image tokens
+        cols = x.to(dt).reshape(b, t, cin, gh, p, gw, p).permute(0, 1, 3, 5, 2, 4, 6).reshape(b * n_img, cin * p * p).contiguous()
+        hidden = torch.empty((b, n, d), dtype=dt, device=x.device)
+        h2 = hidden.view(b * n, d)
+        ctx2 = context.to(dt).reshape(b * tl, -1).contiguous()
+        for bi in range(b):
+            if nt:
+                ops.linear(ctx2[bi * tl + me.start:bi * tl + me.start + nt], *pk["text"], out=h2[bi * n:bi * n + nt])
+            if ni:
+                ops.linear(cols[bi * n_img + i0:bi * n_img + i0 + ni], *pk["patch"], out=h2[bi * n + nt:(bi + 1) * n])
+        e = ops.sinusoidal(timesteps.to(x.device), d, dtype=dt)
+        e = ops.linear(e, *pk["te0"], flags=ops.FLAG_SILU_OUT)
+        emb = ops.linear(e, *pk["te2"])
+        for layer in pk["layers"]:
+            hidden = layer.forward_shard(hidden, emb, sp)
+        # ---- final layer on the shard's image tokens, then one all-gather of them
+        h2 = hidden.reshape(b * n, d)
+        mod = ops.linear(ops.silu(emb), *pk["ada_f"])
+        out = torch.empty((b, ni, p * p * c["out_channels"]), dtype=dt, device=x.device)
+        g, be = pk["norm_final"]
+        for bi in range(b):
+            if not ni:
+                continue
+            img = ops.layernorm(h2[bi * n + nt:(bi + 1) * n], *pk["ln_f"], eps=self.ln_eps)
+            shift, scale = mod[bi, :d].float(), mod[bi, d:].float()
+            img = ops.layernorm(img, (g * (1 + scale)).to(dt), (be * (1 + scale) + shift).to(dt), eps=1e-6)
+            ops.linear(img, *pk["lin_f"], out=out[bi])
+        out = sp.gather_image_rows(out.transpose(0, 1)).transpose(0, 1)             # (b, n_img, p*p*co)
+        co = c["out_channels"]
+        return out.reshape(b, t, gh, gw, co, p, p).permute(0, 1, 4, 2, 5, 3, 6).reshape(b, t, co, gh * p, gw * p)

@@ -707,14 +707,8 @@ liem_reduce_kernel(const __half* __restrict__ x, __half* __restrict__ mm, long l
     }
 }
 // step 2: 7x7 conv (2 -> 1, pad 3, no bias) + sigmoid -> gate[R] fp16.  wt = conv1.weight[0] as [2][7][7]
-__global__ void liem_conv7_kernel(const __half* __restrict__ mm, const __half* __restrict__ wt, __half* __restrict__ gate,
-                                  int BT, int H, int W) {
-    __shared__ float w_s[98];
-    if (threadIdx.x < 98) w_s[threadIdx.x] = __half2float(wt[threadIdx.x]);
-    __syncthreads();
-    const long long n = (long long)BT * H * W;
-    const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-    if (i >= n) return;
+// The gate of token i of the mm map [BT, H, W][2]; w_s = wt in fp32.
+__device__ __forceinline__ __half liem_conv7_gate(const __half* __restrict__ mm, const float* w_s, long long i, int H, int W) {
     const int w0 = (int)(i % W), h0 = (int)((i / W) % H);
     const long long bt = i / ((long long)W * H);
     float acc = 0.f;
@@ -730,7 +724,30 @@ __global__ void liem_conv7_kernel(const __half* __restrict__ mm, const __half* _
         }
     }
     const float a = __half2float(__float2half_rn(acc));      // fp16 conv output in the reference
-    gate[i] = __float2half_rn(sigmoid_f(a));
+    return __float2half_rn(sigmoid_f(a));
+}
+
+__global__ void liem_conv7_kernel(const __half* __restrict__ mm, const __half* __restrict__ wt, __half* __restrict__ gate,
+                                  int BT, int H, int W) {
+    __shared__ float w_s[98];
+    if (threadIdx.x < 98) w_s[threadIdx.x] = __half2float(wt[threadIdx.x]);
+    __syncthreads();
+    const long long n = (long long)BT * H * W;
+    const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    gate[i] = liem_conv7_gate(mm, w_s, i, H, W);
+}
+
+// The same gates for tokens [r0, r0 + n) of the map only (gate[0..n)): a rank of a token-sharded DiT holds the whole
+// map but gates only its own tokens.
+__global__ void liem_conv7_rows_kernel(const __half* __restrict__ mm, const __half* __restrict__ wt, __half* __restrict__ gate,
+                                       int H, int W, long long r0, long long n) {
+    __shared__ float w_s[98];
+    if (threadIdx.x < 98) w_s[threadIdx.x] = __half2float(wt[threadIdx.x]);
+    __syncthreads();
+    const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    gate[i] = liem_conv7_gate(mm, w_s, r0 + i, H, W);
 }
 
 // ------------------------------------------------------------------ CogVideoX DiT helpers (cogvideox-based/sat/dit_video_concat.py)

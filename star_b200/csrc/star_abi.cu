@@ -159,8 +159,10 @@ int make_slab_tmap(CUtensorMap* m, const void* base, long long ld, const TapGemm
 // Launches a tap-GEMM whose caller has filled p's output extents, box, taps, K, N, flags and epilogue inputs.  A holds
 // p.K channels per row, rows lda elements apart, viewed as extents n1..n4 (n1 fastest); W is [N (2N with GEGLU), ntaps * K].
 // Every other field of p, and the tensor maps, follow from those here.
+// a_stride2 (elements, 0 = n1 rows of lda) is the distance between A's n2 slices when they are not packed back to back.
 int launch_tapgemm(TapGemmParams& p, const void* A, unsigned long long lda, unsigned long long n1, unsigned long long n2,
-                   unsigned long long n3, unsigned long long n4, const void* W, cudaStream_t st) {
+                   unsigned long long n3, unsigned long long n4, const void* W, cudaStream_t st,
+                   unsigned long long a_stride2 = 0) {
     long long m_tiles = 1;
     p.box_rows = 1;
     for (int i = 0; i < 4; ++i) {
@@ -185,7 +187,7 @@ int launch_tapgemm(TapGemmParams& p, const void* A, unsigned long long lda, unsi
 
     TapGemmMaps m;
     unsigned long long adim[5] = {(unsigned long long)p.K, n1, n2, n3, n4}, astr[5] = {1, lda};
-    for (int i = 2; i < 5; ++i) astr[i] = astr[i - 1] * adim[i - 1];
+    for (int i = 2; i < 5; ++i) astr[i] = (i == 2 && a_stride2) ? a_stride2 : astr[i - 1] * adim[i - 1];
     unsigned abox[5] = {TG_BK, (unsigned)p.box[0], (unsigned)p.box[1], (unsigned)p.box[2], (unsigned)p.box[3]};
     if (make_tmap(&m.a, A, 5, adim, astr, abox)) return 1;
     const unsigned long long wrows = geglu ? 2ull * p.N : (unsigned long long)p.N;
@@ -285,25 +287,41 @@ int star_init(int device) {
 int star_linear(const void* A, long long lda, const void* W, const void* bias, const void* rowvec,
                 long long rowvec_div, const void* residual, long long ldres, void* out, long long ldo,
                 long long rows, int K, int N, int flags, void* stream) {
-    return star_linear_ex(A, lda, W, bias, rowvec, rowvec_div, nullptr, residual, ldres, out, ldo, rows, K, N, flags, stream);
+    return star_linear_ex(A, lda, W, bias, rowvec, rowvec_div, nullptr, residual, ldres, out, ldo, rows, K, N, flags, 0, 0,
+                          stream);
 }
 
+// A head-blocked A (a_block_cols > 0) is a tap-GEMM with one tap per block: A viewed as (a_block_cols, rows, blocks) with
+// the blocks a_block_pitch apart, tap t shifts to block t, and W's [N, K] columns are the taps' K ranges side by side.  The
+// K loop (taps outer, 64-column chunks inner) thus visits W's columns in the order of the unblocked call, 64 at a time.
 int star_linear_ex(const void* A, long long lda, const void* W, const void* bias, const void* rowvec,
                    long long rowvec_div, const void* colscale, const void* residual, long long ldres, void* out,
-                   long long ldo, long long rows, int K, int N, int flags, void* stream) {
+                   long long ldo, long long rows, int K, int N, int flags, int a_block_cols, long long a_block_pitch,
+                   void* stream) {
     STAR_CHECK_INIT();
     if (rows <= 0) return 0;
     if (K % 8 || lda % 8) return fail("star_linear: K and lda must be multiples of 8 (K=%d lda=%lld)", K, lda);
     if (rows > 0x7fffffffll) return fail("star_linear: too many rows");
+    const int blocks = a_block_cols > 0 ? K / a_block_cols : 1;
+    if (a_block_cols > 0) {
+        if (a_block_cols % TG_BK || K % a_block_cols)
+            return fail("star_linear_ex: a_block_cols (%d) must be a multiple of %d dividing K (%d)", a_block_cols, TG_BK, K);
+        if (blocks > TG_MAX_TAPS) return fail("star_linear_ex: %d A blocks (at most %d)", blocks, TG_MAX_TAPS);
+        if (a_block_pitch % 8 || a_block_pitch < rows * lda)
+            return fail("star_linear_ex: a_block_pitch %lld must be a multiple of 8 and hold %lld rows", a_block_pitch, rows);
+        if (flags & TG_GEGLU) return fail("star_linear_ex: GEGLU does not take a head-blocked A");
+    }
     TapGemmParams p{};
     p.on[0] = (int)rows; p.on[1] = p.on[2] = p.on[3] = 1;
     p.box[0] = TG_BM; p.box[1] = p.box[2] = p.box[3] = 1;
-    p.ntaps = 1;
-    p.K = K; p.N = N; p.flags = flags;
+    p.ntaps = blocks;
+    for (int t = 0; t < blocks; ++t) p.tap[t][1] = t;
+    p.K = a_block_cols > 0 ? a_block_cols : K; p.N = N; p.flags = flags;
     p.bias = (const __half*)bias; p.rowvec = (const __half*)rowvec; p.rowvec_div = (int)rowvec_div;
     p.colscale = (const __half*)colscale; p.residual = (const __half*)residual; p.res_ld = ldres;
     p.out = (__half*)out; p.out_ld = ldo;
-    return launch_tapgemm(p, A, lda, rows, 1, 1, 1, W, (cudaStream_t)stream);
+    return launch_tapgemm(p, A, lda, rows, blocks, 1, 1, W, (cudaStream_t)stream,
+                          a_block_cols > 0 ? (unsigned long long)a_block_pitch : 0ull);
 }
 
 int star_conv2d_3x3(const void* X, const void* W9, const void* bias, const void* rowvec, long long rowvec_div, long long ldrowvec,
@@ -671,15 +689,27 @@ int star_layernorm(const void* X, const void* gamma, const void* beta, void* out
 }
 
 int star_liem_spatial_gate(const void* X, const void* w98, void* mm_ws, void* gate, int BT, int H, int W, int C,
-                           void* stream) {
+                           long long r0, long long n, void* stream) {
     if (C % 8) return fail("star_liem_spatial_gate: C must be a multiple of 8");
     cudaStream_t st = (cudaStream_t)stream;
     const long long rows = (long long)BT * H * W;
-    liem_reduce_kernel<<<(unsigned)std::min<long long>((rows + 7) / 8, (long long)num_sms() * 8), 256, 0, st>>>((const __half*)X, (__half*)mm_ws, rows, C);
-    STAR_LAUNCH_CHECK("liem_reduce");
-    liem_conv7_kernel<<<(unsigned)((rows + 255) / 256), 256, 0, st>>>((const __half*)mm_ws, (const __half*)w98, (__half*)gate,
-                                                                       BT, H, W);
-    STAR_LAUNCH_CHECK("liem_conv7");
+    if (r0 < 0 || n < 0 || r0 + n > rows) return fail("star_liem_spatial_gate: tokens [%lld, %lld) outside the clip's %lld", r0, r0 + n, rows);
+    if (n == 0) return 0;
+    if (X) {
+        liem_reduce_kernel<<<(unsigned)std::min<long long>((n + 7) / 8, (long long)num_sms() * 8), 256, 0, st>>>(
+            (const __half*)X, (__half*)mm_ws + 2 * r0, n, C);
+        STAR_LAUNCH_CHECK("liem_reduce");
+    }
+    if (!gate) return 0;
+    if (r0 == 0 && n == rows) {
+        liem_conv7_kernel<<<(unsigned)((rows + 255) / 256), 256, 0, st>>>((const __half*)mm_ws, (const __half*)w98, (__half*)gate,
+                                                                           BT, H, W);
+        STAR_LAUNCH_CHECK("liem_conv7");
+    } else {
+        liem_conv7_rows_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>((const __half*)mm_ws, (const __half*)w98,
+                                                                             (__half*)gate, H, W, r0, n);
+        STAR_LAUNCH_CHECK("liem_conv7_rows");
+    }
     return 0;
 }
 

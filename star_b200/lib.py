@@ -20,7 +20,7 @@ SIGNATURES = {
     "star_launch_count": (_ll, []),
     "star_init": (_i, [_i]),
     "star_linear": (_i, [_p, _ll, _p, _p, _p, _ll, _p, _ll, _p, _ll, _ll, _i, _i, _i, _p]),
-    "star_linear_ex": (_i, [_p, _ll, _p, _p, _p, _ll, _p, _p, _ll, _p, _ll, _ll, _i, _i, _i, _p]),
+    "star_linear_ex": (_i, [_p, _ll, _p, _p, _p, _ll, _p, _p, _ll, _p, _ll, _ll, _i, _i, _i, _i, _ll, _p]),
     "star_row_gate": (_i, [_p, _p, _ll, _i, _i, _p, _f, _f, _p]),
     "star_qk_ln_rope": (_i, [_p, _ll, _ll, _i, _i, _p, _p, _p, _p, _p, _p, _i, _i, _f, _p]),
     "star_conv2d_3x3": (_i, [_p, _p, _p, _p, _ll, _ll, _p, _ll, _p, _ll, _i, _i, _i, _i, _i, _i, _i, _p]),
@@ -37,7 +37,7 @@ SIGNATURES = {
     "star_groupnorm": (_i, [_p, _p, _p, _p, _i, _ll, _i, _f, _i, _ll, _ll, _ll, _i, _p, _p]),
     "star_groupnorm_mod": (_i, [_p, _p, _p, _p, _p, _ll, _p, _i, _i, _i, _i, _i, _i, _i, _f, _i, _p, _p]),
     "star_layernorm": (_i, [_p, _p, _p, _p, _ll, _i, _f, _i, _p, _f, _f, _p]),
-    "star_liem_spatial_gate": (_i, [_p, _p, _p, _p, _i, _i, _i, _i, _p]),
+    "star_liem_spatial_gate": (_i, [_p, _p, _p, _p, _i, _i, _i, _i, _ll, _ll, _p]),
     "star_concat_add": (_i, [_p, _i, _p, _p, _i, _p, _ll, _p]),
     "star_add": (_i, [_p, _p, _p, _ll, _p]),
     "star_time_avgpool2": (_i, [_p, _p, _i, _ll, _i, _p]),

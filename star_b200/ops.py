@@ -325,16 +325,43 @@ def layernorm(x, gamma, beta, gate_mode=0, gate=None, w0=0.0, w1=0.0, eps=1e-5):
     return out
 
 
+class LiemPart(NamedTuple):
+    """Tokens [r0, r0 + n) of a clip whose channel max / mean map ``liem_spatial_gate(part=)`` reads and writes in mm
+    [BT*H*W, 2]: a token-sharded DiT rank's image tokens."""
+    mm: torch.Tensor
+    r0: int
+    n: int
+
+
 @_traced
-def liem_spatial_gate(x, w98, BT, H, W):
+def liem_spatial_gate(x, w98, BT, H, W, part=None):
+    """gate [BT*H*W] of the clip x [BT*H*W, C].  With part (a LiemPart), the two steps run on the part's tokens only:
+    x (or None) holds their rows [n, C], whose max / mean are written to part.mm; w98 (or None: returns part.mm) gates them
+    from the whole map part.mm, returning their n gates."""
+    if part is not None:
+        return _liem_part(x, w98, BT, H, W, part)
     L, dt = _bind(x)
     rows, C = x.shape
     assert rows == BT * H * W and x.is_contiguous()
     mm = torch.empty((rows, 2), dtype=dt, device=x.device)
     gate = torch.empty((rows,), dtype=dt, device=x.device)
-    _L.check(L, L.star_liem_spatial_gate(_p(x), _p(w98), _p(mm), _p(gate), BT, H, W, C, _st()),
+    _L.check(L, L.star_liem_spatial_gate(_p(x), _p(w98), _p(mm), _p(gate), BT, H, W, C, 0, rows, _st()),
              "star_liem_spatial_gate")
     return gate
+
+
+def _liem_part(x, w98, BT, H, W, part):
+    L, dt = _bind(part.mm)
+    assert part.mm.is_contiguous() and tuple(part.mm.shape) == (BT * H * W, 2)
+    C = 8
+    if x is not None:
+        _h(x, "x", dt)
+        assert x.is_contiguous() and x.shape[0] == part.n
+        C = x.shape[1]
+    gate = torch.empty((part.n,), dtype=dt, device=part.mm.device) if w98 is not None else None
+    _L.check(L, L.star_liem_spatial_gate(_p(x), _p(w98), _p(part.mm), _p(gate), BT, H, W, C, int(part.r0), int(part.n),
+                                         _st()), "star_liem_spatial_gate")
+    return part.mm if gate is None else gate
 
 
 @_traced
@@ -558,17 +585,26 @@ FLAG_GELU_TANH = 8
 
 @_traced
 def linear_ex(a, w, bias=None, colscale=None, residual=None, flags=0, out=None):
-    """out = residual + colscale[n] * act(sum_k a[r,k] w[n,k] + bias[n])   (adaLN-gated residual, tanh-GELU option)"""
+    """out = residual + colscale[n] * act(sum_k a[r,k] w[n,k] + bias[n])   (adaLN-gated residual, tanh-GELU option).
+    a is a strided 2-D view [rows, K], or a head-blocked A: a 3-D view [blocks, rows, block_cols] with contiguous columns
+    whose row r is its blocks' rows r side by side (K = blocks * block_cols), read in place."""
     L, dt = _bind(a)
-    lda = _rowmajor(a, "a")
-    rows, K = a.shape
+    block_cols = pitch = 0
+    if a.dim() == 3:
+        if a.stride(2) != 1:
+            raise _L.StarError("a head-blocked a must have contiguous columns")
+        blocks, rows, block_cols = a.shape
+        lda, pitch, K = a.stride(1), a.stride(0), blocks * block_cols
+    else:
+        lda = _rowmajor(a, "a")
+        rows, K = a.shape
     N = w.shape[0]
     assert w.is_contiguous() and w.shape[1] == K
     if out is None:
         out = torch.empty((rows, N), dtype=dt, device=a.device)
     ldres = _rowmajor(residual, "residual") if residual is not None else 0
     _L.check(L, L.star_linear_ex(_p(a), lda, _p(w), _p(bias), None, 1, _p(colscale), _p(residual), ldres, _p(out),
-                                 _rowmajor(out, "out"), rows, K, N, flags, _st()), "star_linear_ex")
+                                 _rowmajor(out, "out"), rows, K, N, flags, block_cols, pitch, _st()), "star_linear_ex")
     return out
 
 
